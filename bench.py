@@ -1,7 +1,8 @@
 #!/usr/bin/env python3
-"""bench.py — Pallas MSM points/s (+ Fp NTT elements/s) at 2^16 on B200, next to the CPU oracle on the same host.
+"""bench.py — Pallas MSM points/s (+ Fp NTT elements/s) at 2^16 on H100, next to the CPU oracle on the same host.
 
     python bench.py --gpus N --steps K --warmup W            # our arm (CUDA library through its C ABI)
+    python bench.py ... --dump-outputs DIR                   # + what the timed calls returned in their last step, DIR/<name>.npy
     python bench.py --impl reference --gpus N ...            # CPU arm: the oracle port of the reference's ark MSM/FFT
     torchrun --nproc-per-node N bench.py --gpus N ...        # N > 1: one rank per GPU
 
@@ -13,7 +14,7 @@ followed by one 2^16-element Fp NTT.  The headline metric is the MSM's points/s;
 N > 1 (weak scaling): every rank holds the SRS and runs its own 2^16-point slice of an (N * 2^16)-point MSM; the N
 partials stay on the device as c slice sums (128 B each), are exchanged with one NCCL all_gather enqueued behind the kernels and
 summed on the device (proof_systems_b200/parallel.py: ShardedMsm).  NTT: N independent replicas.
-Between timed iterations a 256 MiB buffer is overwritten to flush the 126 MB L2.
+Between timed iterations a 256 MiB buffer is overwritten to flush the 50 MB L2.
 """
 import argparse
 import json
@@ -33,24 +34,19 @@ MSM_BYTES_PER_POINT = 96      # 64 B affine base + 32 B scalar (SURVEY.md §8d)
 NTT_BYTES_PER_ELEM = 64       # 32 B read + 32 B write per transform
 
 
-def load_traffic():
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    return json.load(open(p)) if os.path.exists(p) else {}
-
-
 def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 class ClockSampler:
     """SM clock + clock-event reasons DURING the timed region: one NVML query between every two timed steps, from the main thread,
-    outside the CUDA-event span.  (A polling thread — every 2 ms, then every 10 ms — was measured to stall a step by ~3 ms whenever
-    a query coincided with it: NVML and the CUDA runtime share driver locks, and on an 8-GPU box with 8 ranks one such stall per
-    20-step leg cost 0.17 ms per step on every rank, tools/diag_scale.py.)  nvidia-smi is the fallback when NVML cannot be loaded."""
+    outside the CUDA-event span.  (A polling thread stalls a step by milliseconds whenever a query coincides with it: NVML and the
+    CUDA runtime share driver locks, and with N ranks one such stall is billed to every rank, tools/diag_scale.py.)  nvidia-smi is
+    the fallback when NVML cannot be loaded."""
     NAMES = ("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap")
 
     def __init__(self, index=0):
@@ -130,6 +126,19 @@ def splitmix64_limbs(seed, n):
     return w
 
 
+def limbs_f64(a):
+    """uint64 limb arrays [..., k] -> float64 [..., 2k]: the 32-bit words of every limb, low word first (exact in float64)"""
+    a = np.ascontiguousarray(a, dtype=np.uint64)
+    return a.view("<u4").reshape(a.shape[:-1] + (2 * a.shape[-1],)).astype(np.float64)
+
+
+def dump_outputs(out_dir, arrays):
+    """--dump-outputs: one float64 .npy per output (field elements and affine points as 32-bit words, see limbs_f64)"""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), limbs_f64(a))
+
+
 def compressed_srs():
     """the reference's own srs/pallas.srs generators (compressed, 33 B each), via tests/golden"""
     return np.load(os.path.join(ROOT, "tests", "golden", "pallas_srs.npz"))["g_cmp"]
@@ -160,7 +169,7 @@ def cpu_msm(orc, g, scalars, threads):
 
 
 def best_threads(fn, max_threads):
-    """The GPU boxes expose 64-128 hardware threads that are not always all usable (shared host, cgroup quota): after one untimed
+    """A GPU host's hardware threads are not always all usable (shared host, cgroup quota): after one untimed
     warm-up (OpenMP pool start-up, page faults), run the CPU arm twice per candidate thread count and keep the count with the best
     of its two runs — the baseline gets its best configuration, picked from warmed measurements."""
     best, best_t = None, None
@@ -234,6 +243,8 @@ def main():
     ap.add_argument("--window-bits", type=int, default=16, help="table window of the resident SRS for the headline (16 = BASELINE config 2's w; -1: library default)")
     ap.add_argument("--cpu-seconds", type=float, default=6.0, help="budget of the cpu_baseline leg")
     ap.add_argument("--no-extra", action="store_true", help="skip the cfg1 / cfg3 / cfg4 legs (tools/ use this for quick A/B runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what every timed call returned in its last step as "
+                    "DIR/<name>.npy (float64; MSM results as affine points, 2^20-element outputs as a fixed sample of 2^16 rows)")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3
@@ -283,7 +294,7 @@ def main():
             torch.cuda.synchronize()
             if world > 1 and collective:
                 # every rank enters the step together: the untimed flush / host work of the slowest rank must not be billed to the
-                # others' collective (at N = 8 that skew was +0.3 ms per step); the rendezvous itself is outside the event span
+                # others' collective; the rendezvous itself is outside the event span
                 dist.barrier()
                 torch.cuda.synchronize()
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -324,6 +335,15 @@ def main():
     # enqueues ONE ncclAllGather of N x c x 128 bytes from C on the context's stream behind the kernels, adds the partials on the
     # device and reads them back once.  torch.distributed only carried the 128-byte NCCL id at start-up.
     comm = LibraryComm(ctx) if world > 1 else None
+    # what the timed calls returned in their most recent step (--dump-outputs): MSM Jacobian points by name, other arrays as is
+    last_jac, last_arrays = {}, {}
+
+    def kept(name, curve, fn):
+        def step():
+            r = fn()
+            last_jac[name] = (curve, r)
+            return r
+        return step
 
     def msm_host(b, h_sc, n):
         out = np.empty(12, dtype=np.uint64)
@@ -354,13 +374,15 @@ def main():
         ntt_e2e()
     barrier()
     launches0 = ctx.launch_count
-    msm_ms = timed(step_resident, args.steps, collective=True)
+    msm_ms = timed(kept("msm", zk.PALLAS, step_resident), args.steps, collective=True)
     barrier()
     ntt_ms = timed(ntt_resident, args.steps)
+    last_arrays["ntt"] = d_poly.cpu().numpy().view(np.uint64).reshape(N_PTS, 4)      # the transforms are in place
     barrier()
-    msm_e2e_ms = timed(step_e2e, args.steps, collective=True)
+    msm_e2e_ms = timed(kept("msm_e2e", zk.PALLAS, step_e2e), args.steps, collective=True)
     barrier()
     ntt_e2e_ms = timed(ntt_e2e, args.steps)
+    last_arrays["ntt_e2e"] = h_poly.numpy().view(np.uint64).reshape(N_PTS, 4).copy()
     barrier()
     launches_total = ctx.launch_count - launches0
 
@@ -394,7 +416,6 @@ def main():
     msm_e2e_ms, ntt_e2e_ms = max_over_ranks(msm_e2e_ms), max_over_ranks(ntt_e2e_ms)
 
     peak, peak_src = load_peaks()
-    traffic = load_traffic()
     extra = {"table_build_ms": {f"pallas_2^16_w{wb}": round(table_ms, 3)}}
     ok_all = True
 
@@ -403,8 +424,8 @@ def main():
         b2, t2 = upload_timed(zk.PALLAS, g, -1)
         for _ in range(3):
             r2 = ctx.msm_dev(b2, d_scalars.data_ptr(), N_PTS)
-        t_res = timed(lambda: ctx.msm_dev(b2, d_scalars.data_ptr(), N_PTS), args.steps) / args.steps
-        t_e2e = timed(lambda: msm_host(b2, h_scalars, N_PTS), args.steps) / args.steps
+        t_res = timed(kept("tuned_window_msm", zk.PALLAS, lambda: ctx.msm_dev(b2, d_scalars.data_ptr(), N_PTS)), args.steps) / args.steps
+        t_e2e = timed(kept("tuned_window_msm_e2e", zk.PALLAS, lambda: msm_host(b2, h_scalars, N_PTS)), args.steps) / args.steps
         a2, st2 = stage_profile(lambda: ctx.msm_dev(b2, d_scalars.data_ptr(), N_PTS), 5)
         same = bool(np.array_equal(zk.jacobian_to_affine(zk.PALLAS, r2), zk.jacobian_to_affine(zk.PALLAS, result)))
         ok_all &= same
@@ -417,8 +438,8 @@ def main():
         b1 = ctx.upload_bases(zk.PALLAS, g[:n1], window_bits=-1)
         for _ in range(3):
             r1 = ctx.msm_dev(b1, d_scalars.data_ptr(), n1)
-        t1 = timed(lambda: ctx.msm_dev(b1, d_scalars.data_ptr(), n1), args.steps) / args.steps
-        t1e = timed(lambda: msm_host(b1, h_scalars, n1), args.steps) / args.steps
+        t1 = timed(kept("cfg1_msm", zk.PALLAS, lambda: ctx.msm_dev(b1, d_scalars.data_ptr(), n1)), args.steps) / args.steps
+        t1e = timed(kept("cfg1_msm_e2e", zk.PALLAS, lambda: msm_host(b1, h_scalars, n1)), args.steps) / args.steps
         _, st1 = stage_profile(lambda: ctx.msm_dev(b1, d_scalars.data_ptr(), n1), 5)
         extra["cfg1_pallas_2^11"] = {"workload": "2^11-point Pallas MSM on srs/pallas.srs generators (BASELINE config 1)", "window_bits": b1.window_bits,
                                      "ms_per_step": t1, "value": n1 / (t1 * 1e-3), "e2e_ms_per_step": t1e, "stage_ms": st1, "_result": r1}
@@ -440,19 +461,20 @@ def main():
         rt_ms = max_over_ranks(timed(roundtrip, args.steps)) / args.steps
         stream.synchronize()
         rt_exact = bool(torch.equal(d3, d3_0))
+        rows = torch.from_numpy(np.sort(np.random.default_rng(3).choice(n3, N_PTS, replace=False))).to(dev)
+        last_arrays["cfg3_roundtrip_sample"] = d3[rows].cpu().numpy().view(np.uint64).reshape(N_PTS, 4)
         ctx.ntt_dev(zk.FP, d3.data_ptr(), L3)
         stream.synchronize()                      # the library runs on `stream`; torch's copy below does not
         fwd3 = d3.cpu().numpy().view(np.uint64).reshape(n3, 4)
         d3.copy_(d3_0)
         k3 = ntt_profile(lambda: ctx.ntt_dev(zk.FP, d3.data_ptr(), L3), 5)
         ach3 = NTT_BYTES_PER_ELEM * n3 / (k3 * 1e-3) / 1e9
-        tr20 = traffic.get("k_ntt_pass_2_20", {})
         extra["cfg3_fp_ntt_2^20"] = {
             "workload": "2^20-element Fp NTT forward + inverse round trip (BASELINE config 3)" + ("" if world == 1 else f", {world} replicas"),
             "ms_per_round_trip": rt_ms, "value": world * 2 * n3 / (rt_ms * 1e-3), "unit": "elements/s (2 transforms per round trip)",
             "round_trip_bit_exact": rt_exact,
             "roofline": {"bound": "hbm", "kernel": "k_ntt_pass x2 (one forward transform)", "achieved": ach3, "peak": peak, "unit": "GB/s", "frac": ach3 / peak,
-                         "traffic": (tr20.get("bytes_per_launch", 0) * tr20.get("launches_per_transform", 0)) or None, "kernel_ms": k3,
+                         "traffic": None, "kernel_ms": k3,
                          "algorithmic_bytes": NTT_BYTES_PER_ELEM * n3}}
         ok_all &= rt_exact
         del d3, d3_0
@@ -468,13 +490,12 @@ def main():
         d_sc4 = torch.from_numpy(sc4[lo:hi].view(np.int64)).cuda()
         h_sc4 = torch.from_numpy(sc4[lo:hi].view(np.int64).copy()).pin_memory()
         sh4 = comm.msm if comm else (lambda bb, ptr, cnt: ctx.msm_dev(bb, ptr, cnt) if ptr == d_sc4.data_ptr() else msm_host(bb, h_sc4, cnt))
-        steps4 = max(3, min(args.steps, 10))
         for _ in range(3):
             r4 = sh4(b4, d_sc4.data_ptr(), hi - lo)
         barrier()
-        t4_res = max_over_ranks(timed(lambda: sh4(b4, d_sc4.data_ptr(), hi - lo), steps4, collective=True)) / steps4
+        t4_res = max_over_ranks(timed(kept("cfg4_msm", zk.VESTA, lambda: sh4(b4, d_sc4.data_ptr(), hi - lo)), args.steps, collective=True)) / args.steps
         barrier()
-        t4_e2e = max_over_ranks(timed(lambda: sh4(b4, h_sc4.data_ptr(), hi - lo), steps4, collective=True)) / steps4
+        t4_e2e = max_over_ranks(timed(kept("cfg4_msm_e2e", zk.VESTA, lambda: sh4(b4, h_sc4.data_ptr(), hi - lo)), args.steps, collective=True)) / args.steps
         barrier()
         a4, st4 = stage_profile(lambda: ctx.msm_dev(b4, d_sc4.data_ptr(), hi - lo), 3)
         ach4 = MSM_BYTES_PER_POINT * (hi - lo) / (a4 * 1e-3) / 1e9
@@ -495,6 +516,8 @@ def main():
         if world > 1:
             dist.destroy_process_group()
         return
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {**{k: zk.jacobian_to_affine(c, r) for k, (c, r) in last_jac.items()}, **last_arrays})
 
     # ---- correctness of what was timed + CPU baseline on the same host (bounded sample): the only use of the oracle
     from oracle import oracle as orc
@@ -535,9 +558,6 @@ def main():
         c4["result_matches_cpu_oracle"] = bool(np.array_equal(zk.jacobian_to_affine(zk.VESTA, r4), w4))
         ok_all &= c4["result_matches_cpu_oracle"]
 
-    msm_traffic = traffic.get(f"k_accumulate_w{wb}", traffic.get("k_accumulate", {}) if wb == 15 else {}).get("bytes_per_launch")
-    ntt_traffic = traffic.get("k_ntt_pass", {})
-    ntt_traffic = ntt_traffic.get("bytes_per_launch", 0) * ntt_traffic.get("launches_per_transform", 0) or None
     per_step_ms = msm_ms / args.steps
     value = world * N_PTS / (per_step_ms * 1e-3)
     e2e_value = world * N_PTS / (msm_e2e_ms / args.steps * 1e-3)
@@ -556,10 +576,10 @@ def main():
         "gpu_launches": int(launches_total),
         "clocks": clocks,
         "roofline": {"bound": "hbm", "kernel": "k_accumulate (bucket accumulation)", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                     "frac": achieved / peak, "traffic": msm_traffic, "peak_source": peak_src, "kernel_ms": acc_ms,
+                     "frac": achieved / peak, "traffic": None, "peak_source": peak_src, "kernel_ms": acc_ms,
                      "algorithmic_bytes": MSM_BYTES_PER_POINT * N_PTS,
                      "note": "MSM is integer-ALU bound: 96 B/point of compulsory traffic vs ~16 mixed additions (~190 modular multiplications) per point; "
-                             "the accumulation kernel gathers 64 B per (point, window) from the resident table, which is what `traffic` shows",
+                             "the accumulation kernel gathers 64 B per (point, window) from the resident table",
                      "stage_ms": stages},
         "cpu_baseline": {"value": N_PTS / cpu_msm_s, "unit": "points/s", "cores": threads, "kind": "port",
                          "sample": f"{cpu_reps} x the same 2^16-point MSM (oracle: ark-style Pippenger, 2-way split, best of 8..{orc.host_threads()} threads = {threads}), {cpu_msm_s * 1e3:.1f} ms each"},
@@ -567,7 +587,7 @@ def main():
             "metric": "fp_ntt_elements_per_s", "workload": "2^16-element Fp forward NTT (Radix2EvaluationDomain::fft_in_place)" + ("" if world == 1 else f", {world} replicas"),
             "value": world * N_PTS / (ntt_ms / args.steps * 1e-3), "unit": "elements/s", "ms_per_step": ntt_ms / args.steps,
             "e2e": {"value": world * N_PTS / (ntt_e2e_ms / args.steps * 1e-3), "unit": "elements/s", "h2d_bytes_per_step": N_PTS * 32, "d2h_bytes_per_step": N_PTS * 32},
-            "roofline": {"bound": "hbm", "kernel": "k_ntt_pass x2", "achieved": ntt_ach, "peak": peak, "unit": "GB/s", "frac": ntt_ach / peak, "traffic": ntt_traffic, "kernel_ms": ntt_k,
+            "roofline": {"bound": "hbm", "kernel": "k_ntt_pass x2", "achieved": ntt_ach, "peak": peak, "unit": "GB/s", "frac": ntt_ach / peak, "traffic": None, "kernel_ms": ntt_k,
                          "algorithmic_bytes": NTT_BYTES_PER_ELEM * N_PTS},
             "cpu_baseline": {"value": N_PTS / cpu_ntt_s, "unit": "elements/s", "cores": threads, "kind": "port", "sample": f"{cpu_ntt_reps} x the same transform"},
         },

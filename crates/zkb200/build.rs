@@ -1,4 +1,4 @@
-// Links libzkb200.so (built by `make -C proof_systems_b200/csrc`, nvcc -gencode arch=compute_100a,code=sm_100a).
+// Links libzkb200.so (built by `make -C proof_systems_b200/csrc`, nvcc -gencode arch=compute_90a,code=sm_90a).
 // ZKB200_LIB_DIR: directory holding libzkb200.so (default: ../../proof_systems_b200 relative to this crate).
 use std::{env, path::PathBuf};
 

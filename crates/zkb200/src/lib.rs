@@ -1,4 +1,4 @@
-//! B200 back end for Kimchi's two proving-time hot paths, behind the reference's own seams:
+//! H100 back end for Kimchi's two proving-time hot paths, behind the reference's own seams:
 //!
 //! * [`GpuSRS`] implements `poly_commitment::SRS<G>` (poly-commitment/src/lib.rs:61-241) — every MSM-bearing method runs on the
 //!   device, the rest follows `ipa::SRS` (poly-commitment/src/ipa.rs:596-800);

@@ -1,5 +1,5 @@
 /*
- * zkb200.h — C ABI of the B200-native MSM + NTT hot path of o1-labs/proof-systems (Kimchi).
+ * zkb200.h — C ABI of the H100-native MSM + NTT hot path of o1-labs/proof-systems (Kimchi).
  *
  * The reference has NO C ABI or plugin loader on this path: its seam is two Rust traits and one arkworks trait
  * (SURVEY.md §8b).  These entry points are what a Rust `extern "C"` block behind those traits binds

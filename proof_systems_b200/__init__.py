@@ -1,6 +1,6 @@
-"""proof_systems_b200 — B200-native MSM + NTT hot path of o1-labs/proof-systems (Kimchi).
+"""proof_systems_b200 — H100-native MSM + NTT hot path of o1-labs/proof-systems (Kimchi).
 
-The product is the C-ABI shared library `libzkb200.so` (include/zkb200.h; hand-written sm_100a CUDA kernels under
+The product is the C-ABI shared library `libzkb200.so` (include/zkb200.h; hand-written sm_90a CUDA kernels under
 csrc/).  This package is the thin Python host layer used by the tests and bench.py: ctypes bindings plus mirrors of the
 reference's interfaces on this path, with the reference's names:
 

@@ -1,4 +1,4 @@
-// field.cuh — 255-bit Pasta field arithmetic for sm_100a: 8 x u32 limbs, Montgomery form (R = 2^256).
+// field.cuh — 255-bit Pasta field arithmetic for sm_90a: 8 x u32 limbs, Montgomery form (R = 2^256).
 //
 // Replaces, on the device, what the reference gets from ark-ff's Fp256<MontBackend<_,4>> (crate not in the
 // reference tree; constants from curves/src/pasta/fields/fp.rs:8-80 and fq.rs:8-79).  The in-memory format is
@@ -233,10 +233,9 @@ template <class F> ZK_HD void mont_reduce_row(uint32_t (&P)[9], uint32_t (&S)[9]
 
 // ZK_MUL_PLAIN_PER_ROW — pipe-balancing experiment prepared for the next GPU round (DESIGN.md "next levers"); 0 = the shipped,
 // measured form (the macro below then expands to exactly the original instruction sequence).  K = 1..6: the K highest products
-// a_j * b_i of every row (j = 7, 6, 5, ...) become PLAIN wide multiplies — 2.1 cycles on the FMA pipe instead of 4.0 for the
-// carry-chained form, and off the carry chains — added in with two carry adds each on the half-idle ALU pipe.  Bit-exact in every
-// setting (tests/test_device_math_host.py builds them all).  SASS of one product (IMAD.WIDE.U32.X / IMAD.WIDE.U32 / IADD3.X):
-//   K = 0: 69 / 21 / 63     K = 2: 55 / 35 / 91     K = 5: 34 / 56 / 133 (both pipes at about 300 cycles by the measured rates)
+// a_j * b_i of every row (j = 7, 6, 5, ...) become PLAIN wide multiplies — cheaper on the FMA pipe than the carry-chained form
+// (tools/ubench/pipes.cu measures both), and off the carry chains — added in with two carry adds each on the ALU pipe.  Bit-exact in
+// every setting (tests/test_device_math_host.py builds them all).
 #ifndef ZK_MUL_PLAIN_PER_ROW
 #define ZK_MUL_PLAIN_PER_ROW 0
 #endif

@@ -1,15 +1,15 @@
-// msm.cuh — variable-base multi-scalar multiplication on Pallas / Vesta for sm_100a.
+// msm.cuh — variable-base multi-scalar multiplication on Pallas / Vesta for sm_90a.
 //
 // Drop-in semantics of ark_ec::VariableBaseMSM::{msm_bigint, msm} as the reference calls them
 // (poly-commitment/src/ipa.rs:649-672,943,953,487,497; commitment.rs:382,387 — SURVEY.md §8 rows a1/a2):
 //     result = sum_i s_i * P_i       bases affine (x, y Montgomery; identity allowed), scalars canonical 255-bit
 // (or Montgomery, converted on the device first), min(len) semantics for msm_bigint.
 //
-// B200 shape (Pippenger with signed digits, bucket method):
+// H100 shape (Pippenger with signed digits, bucket method):
 //   * resident bases: an SRS (or a Lagrange basis) is uploaded once and kept in HBM — optionally as a
 //     PRECOMPUTED table T[w][i] = 2^(c*w) * P_i (nwin * n affine points; 64 MiB for n = 2^16, c = 16).  With the table
 //     all windows share ONE bucket set, so there is no per-window bucket reduction and no Horner doubling chain:
-//     180 GB of HBM buys away ~half of the serial tail.  Without a table (one-shot bases) there is one bucket set per
+//     80 GB of HBM buys away ~half of the serial tail.  Without a table (one-shot bases) there is one bucket set per
 //     window and the host combines the windows.
 //   * scalars are recoded to signed base-2^c digits in (-2^(c-1), 2^(c-1)]; (digit != 0) entries are counting-sorted by
 //     bucket (histogram -> scan -> scatter, all on device);
@@ -74,7 +74,7 @@ struct MsmWorkspace {
     uint32_t chunk = 0;               // K override (0: chosen per call so that the tasks fill the machine once)
     uint32_t wave_threads = 0;        // accumulation threads per SM the task count is sized for (0: built-in default)
     bool tma_gather = false;          // A/B switch: gather the points with the bulk asynchronous copy engine (k_accumulate_tma)
-    int sm_count = 148;               // SMs of the device (set by the context)
+    int sm_count = 132;               // SMs of the device (set by the context)
     bool profile = false;             // record an event after every stage
     cudaEvent_t ev[8] = {};           // MSM_ST_COUNT + 1 stage boundaries
     float stage_ms[8] = {};           // duration of each stage in the last profiled call

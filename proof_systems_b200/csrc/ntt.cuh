@@ -1,4 +1,4 @@
-// ntt.cuh — radix-2 number-theoretic transform over the Pasta fields on sm_100a.
+// ntt.cuh — radix-2 number-theoretic transform over the Pasta fields on sm_90a.
 //
 // Drop-in semantics of ark_poly::Radix2EvaluationDomain::<F>::{fft_in_place, ifft_in_place} as the reference calls
 // them (kimchi/src/prover.rs:289,377,907,1163; kimchi/src/circuits/constraints.rs:494;
@@ -7,9 +7,9 @@
 // natural order in and out, w = (5^T)^(2^(32-log n)) (fp.rs:10,21-27), g = 1 (plain domain) or 5 (coset),
 // elements in Montgomery form, inputs shorter than the domain zero-padded.
 //
-// B200 shape: a four-step decomposition n = n1 * n2 (n1, n2 <= 2^10) makes a transform of up to 2^20 elements exactly two kernel
+// H100 shape: a four-step decomposition n = n1 * n2 (n1, n2 <= 2^10) makes a transform of up to 2^20 elements exactly two kernel
 // passes, n = n1 * n2 * n3 three (up to 2^30).  A pass is a batch of independent S-point column transforms; ONE column is one
-// CTA's tile (32 KiB for S = 1024), so a 2^20 transform is 1024 tiles per pass — fine-grained enough to keep 148 SMs evenly
+// CTA's tile (32 KiB for S = 1024), so a 2^20 transform is 1024 tiles per pass — fine-grained enough to keep 132 SMs evenly
 // loaded, and the 32-byte elements are exactly one DRAM sector each, so strided columns cost no bandwidth.  Inside a tile the
 // transform is decimation in time: the load writes the column to shared memory in bit-reversed order, a warp runs the six
 // layers of span <= 32 for a 64-row chunk entirely in REGISTERS (two elements per lane, partners exchanged with warp shuffles,

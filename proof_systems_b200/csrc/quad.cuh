@@ -1,8 +1,8 @@
 // quad.cuh — latency-optimised XYZZ point addition: FOUR lanes cooperate on ONE addition.
 //
 // The reduction tails of the MSM (per-bucket sums of task partials, bit-sliced bucket sums) are chains of DEPENDENT
-// point additions executed by very few warps; a serial add-2008-s is 14 field multiplications back to back (~4.5 us at
-// one warp per scheduler on B200).  Its data-flow is only four multiplications deep, so a quad computes
+// point additions executed by very few warps; a serial add-2008-s is 14 field multiplications back to back (several
+// microseconds at one warp per scheduler).  Its data-flow is only four multiplications deep, so a quad computes
 //     stage 1   U1 = X1*ZZ2     U2 = X2*ZZ1     S1 = Y1*ZZZ2      S2 = Y2*ZZZ1
 //     stage 2   PP = P^2        RR = R^2        ZZ12 = ZZ1*ZZ2    ZZZ12 = ZZZ1*ZZZ2        (P = U2-U1, R = S2-S1)
 //     stage 3   PPP = P*PP      Q = U1*PP       ZZ3 = ZZ12*PP     W = ZZZ12*P

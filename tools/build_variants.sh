@@ -10,10 +10,10 @@ for spec in "$@"; do
   dir=/tmp/zkb_build_$tag; mkdir -p $dir
   for f in api msm ntt srs group_ntt decompress ipa open $EXTRA_SRCS; do
     [ -f $f.cu ] || continue
-    $NVCC -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -Xcompiler -fPIC,-fvisibility=hidden -ccbin /usr/bin/g++ \
+    $NVCC -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -Xcompiler -fPIC,-fvisibility=hidden -ccbin /usr/bin/g++ \
       --expt-relaxed-constexpr $flags -c -o $dir/$f.o $f.cu &
   done
   wait
-  $NVCC -gencode arch=compute_100a,code=sm_100a -shared -o ../libzkb200_$tag.so $dir/*.o -Xcompiler -fPIC -lcudart
+  $NVCC -gencode arch=compute_90a,code=sm_90a -shared -o ../libzkb200_$tag.so $dir/*.o -Xcompiler -fPIC -lcudart
   echo "built libzkb200_$tag.so"
 done

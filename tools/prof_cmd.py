@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""The command ncu wraps for profiles/: a few 2^16-point Pallas MSMs (table window from argv[1], default 16), a few 2^20 and 2^16
+"""A workload to run under a profiler: a few 2^16-point Pallas MSMs (table window from argv[1], default 16), a few 2^20 and 2^16
 Fp NTTs, device-resident inputs, nothing else on the GPU."""
 import os, sys
 import numpy as np, torch
@@ -7,7 +7,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import proof_systems_b200 as zk
 from bench import splitmix64_limbs
-tma_ab = len(sys.argv) > 1 and sys.argv[1] == "msm_tma"      # alternate the two accumulate kernels (profiles/r02_tma_ab.md)
+tma_ab = len(sys.argv) > 1 and sys.argv[1] == "msm_tma"      # alternate the two accumulate kernels
 if tma_ab: sys.argv[1] = "16"
 wb = int(sys.argv[1]) if len(sys.argv) > 1 else 16
 reps = int(sys.argv[2]) if len(sys.argv) > 2 else 3

@@ -1,5 +1,5 @@
-// tools/ubench/pipes.cu — issue-rate probes for the integer instructions fe_mul is made of (sm_100a).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o pipes pipes.cu ;  run: ./pipes
+// tools/ubench/pipes.cu — issue-rate probes for the integer instructions fe_mul is made of (sm_90a).
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o pipes pipes.cu ;  run: ./pipes
 // Prints warp-instructions per clock per SM for: IMAD.WIDE.U32 (independent), IMAD.WIDE.U32.X carry chains,
 // IADD3 (independent), IADD3.X carry chains, and a 1:1 mix.  Diagnostic only (DESIGN.md compute model).
 #include <cstdint>
