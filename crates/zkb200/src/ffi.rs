@@ -39,6 +39,25 @@ pub struct zk_open_transcript {
     pub final_challenge: unsafe extern "C" fn(user: *mut c_void, delta_xy: *const u64, out_c: *mut u64) -> c_int,
 }
 
+#[repr(C)]
+pub struct zk_verify_proof {
+    pub lr_xy: *const u64,
+    pub n_rounds: usize,
+    pub delta_xy: *const u64,
+    pub z1: *const u64,
+    pub z2: *const u64,
+    pub sg_xy: *const u64,
+    pub elm: *const u64,
+    pub n_elm: usize,
+    pub polyscale: *const u64,
+    pub evalscale: *const u64,
+    pub comm_xy: *const u64,
+    pub comm_chunks: *const usize,
+    pub n_comms: usize,
+    pub combined_inner_product: *const u64,
+    pub transcript: *const zk_open_transcript,
+}
+
 pub const ZK_EXPR_CONST: u32 = 0;
 pub const ZK_EXPR_CELL: u32 = 1;
 pub const ZK_EXPR_DUP: u32 = 2;
@@ -86,6 +105,8 @@ extern "C" {
                        polyscale: *const u64, evalscale: *const u64, rng_scalars: *const u64, n_rng_scalars: usize,
                        transcript: *const zk_open_transcript, out_lr_xy: *mut u64, lr_capacity_rounds: usize, out_rounds: *mut usize,
                        out_delta_xy: *mut u64, out_z1: *mut u64, out_z2: *mut u64, out_sg_xy: *mut u64) -> c_int;
+    pub fn zk_srs_verify(srs: *mut zk_srs, batch: *const zk_verify_proof, n: usize, rng_scalars: *const u64, out_ok: *mut c_int,
+                         out_sum_xyz: *mut u64) -> c_int;
 
     pub fn zk_dev_alloc(ctx: *mut zk_ctx, bytes: usize, out: *mut *mut c_void) -> c_int;
     pub fn zk_dev_free(ctx: *mut zk_ctx, d_ptr: *mut c_void) -> c_int;

@@ -27,9 +27,10 @@ use serde::{Deserialize, Serialize};
 #[serde(bound = "G: ark_serialize::CanonicalDeserialize + ark_serialize::CanonicalSerialize")]
 pub struct GpuOpeningProof<G: AffineRepr, const FULL_ROUNDS: usize>(pub OpeningProof<G, FULL_ROUNDS>);
 
-/// What the three callbacks share: the caller's sponge, its group map and the curve's endo coefficient.
+/// What the three callbacks share: the caller's sponge (the one of `open`, or one batch element's of `verify`), its group map and
+/// the curve's endo coefficient.
 struct Transcript<'a, G: GpuCurve, S, const FULL_ROUNDS: usize> {
-    sponge: S,
+    sponge: &'a mut S,
     group_map: &'a G::Map,
     endo_r: G::ScalarField,
 }
@@ -62,7 +63,7 @@ where
     // ipa.rs:962-970
     t.sponge.absorb_g(&[l]);
     t.sponge.absorb_g(&[r]);
-    let u = squeeze_prechallenge(&mut t.sponge).to_field(&t.endo_r);
+    let u = squeeze_prechallenge(&mut *t.sponge).to_field(&t.endo_r);
     core::slice::from_raw_parts_mut(out_u, 4).copy_from_slice(&G::scalar_limbs(&[u]));
     0
 }
@@ -138,7 +139,8 @@ where
         let draws: Vec<G::ScalarField> = (0..2 * rounds + 2).map(|_| G::ScalarField::rand(rng)).collect();
         let draws = G::scalar_limbs(&draws);
 
-        let mut t = Transcript::<G, EFqSponge, FULL_ROUNDS> { sponge, group_map, endo_r };
+        let mut sponge = sponge;
+        let mut t = Transcript::<G, EFqSponge, FULL_ROUNDS> { sponge: &mut sponge, group_map, endo_r };
         let tr = zk_open_transcript {
             user: (&mut t as *mut Transcript<G, EFqSponge, FULL_ROUNDS>).cast(),
             u_base: cb_u_base::<G, EFqSponge, FULL_ROUNDS>,
@@ -167,8 +169,9 @@ where
         })
     }
 
-    /// Verification is the reference's (ipa.rs:268-533 through `OpeningProof::verify`): its MSM is one 2^16-point call per batch and
-    /// not on the proving-time path.
+    /// `verify` = one `zk_srs_verify` call (csrc/verify.cu): SRS::verify (ipa.rs:301-502) with the challenge polynomials of the
+    /// whole batch expanded on the device and both MSMs there; each element's sponge stays here, behind the same three callbacks as
+    /// `open`, called proof by proof in the reference's order.
     fn verify<EFqSponge, RNG>(
         srs: &Self::SRS,
         group_map: &G::Map,
@@ -179,11 +182,74 @@ where
         EFqSponge: FqSponge<G::BaseField, G, G::ScalarField, FULL_ROUNDS>,
         RNG: RngCore + CryptoRng,
     {
-        // `GpuOpeningProof` is a #[repr(transparent)] newtype of `OpeningProof` and `BatchEvaluationProof` only holds a REFERENCE to
-        // its opening, so the two instantiations of the batch element have the same layout: reinterpret the slice in place
-        // (the sponge is not `Clone` in this signature, so the elements cannot be rebuilt).
-        let inner: &mut [BatchEvaluationProof<G, EFqSponge, OpeningProof<G, FULL_ROUNDS>, FULL_ROUNDS>] =
-            unsafe { core::slice::from_raw_parts_mut(batch.as_mut_ptr().cast(), batch.len()) };
-        srs.inner.verify(group_map, inner, rng)
+        let (_endo_q, endo_r) = endos::<G>();
+        // the reference's draws, in its order (ipa.rs:357-358)
+        let rand_base = G::ScalarField::rand(rng);
+        let sg_rand_base = G::ScalarField::rand(rng);
+        let rng_l = G::scalar_limbs(&[rand_base, sg_rand_base]);
+
+        // per element: limb copies of the proof and its evaluations (they live until the call returns) and a transcript over its sponge
+        struct Limbs {
+            lr: Vec<u64>,
+            delta: [u64; 8],
+            sg: [u64; 8],
+            z: Vec<u64>,
+            elm: Vec<u64>,
+            scales: Vec<u64>,
+            comm: Vec<u64>,
+            chunks: Vec<usize>,
+            cip: Vec<u64>,
+        }
+        let mut limbs: Vec<Limbs> = Vec::with_capacity(batch.len());
+        let mut ts: Vec<Transcript<G, EFqSponge, FULL_ROUNDS>> = Vec::with_capacity(batch.len());
+        for BatchEvaluationProof { sponge, evaluation_points, polyscale, evalscale, evaluations, opening, combined_inner_product } in batch.iter_mut() {
+            let op = &opening.0;
+            limbs.push(Limbs {
+                lr: op.lr.iter().flat_map(|(l, r)| l.limbs().into_iter().chain(r.limbs())).collect(),
+                delta: op.delta.limbs(),
+                sg: op.sg.limbs(),
+                z: G::scalar_limbs(&[op.z1, op.z2]),
+                elm: G::scalar_limbs(evaluation_points),
+                scales: G::scalar_limbs(&[*polyscale, *evalscale]),
+                comm: evaluations.iter().flat_map(|e| e.commitment.chunks.iter().flat_map(|c| c.limbs())).collect(),
+                chunks: evaluations.iter().map(|e| e.commitment.chunks.len()).collect(),
+                cip: G::scalar_limbs(&[*combined_inner_product]),
+            });
+            ts.push(Transcript { sponge, group_map, endo_r });
+        }
+        let trs: Vec<zk_open_transcript> = ts
+            .iter_mut()
+            .map(|t| zk_open_transcript {
+                user: (t as *mut Transcript<G, EFqSponge, FULL_ROUNDS>).cast(),
+                u_base: cb_u_base::<G, EFqSponge, FULL_ROUNDS>,
+                round: cb_round::<G, EFqSponge, FULL_ROUNDS>,
+                final_challenge: cb_final::<G, EFqSponge, FULL_ROUNDS>,
+            })
+            .collect();
+        let descs: Vec<zk_verify_proof> = limbs
+            .iter()
+            .zip(trs.iter())
+            .map(|(l, tr)| zk_verify_proof {
+                lr_xy: l.lr.as_ptr(),
+                n_rounds: l.lr.len() / 16,
+                delta_xy: l.delta.as_ptr(),
+                z1: l.z.as_ptr(),
+                z2: l.z[4..].as_ptr(),
+                sg_xy: l.sg.as_ptr(),
+                elm: l.elm.as_ptr(),
+                n_elm: l.elm.len() / 4,
+                polyscale: l.scales.as_ptr(),
+                evalscale: l.scales[4..].as_ptr(),
+                comm_xy: l.comm.as_ptr(),
+                comm_chunks: l.chunks.as_ptr(),
+                n_comms: l.chunks.len(),
+                combined_inner_product: l.cip.as_ptr(),
+                transcript: tr,
+            })
+            .collect();
+        let mut ok: c_int = 0;
+        check(unsafe { zk_srs_verify(srs.dev.0, descs.as_ptr(), descs.len(), rng_l.as_ptr(), &mut ok, core::ptr::null_mut()) })
+            .expect("zkb200: verify");
+        ok != 0
     }
 }

@@ -19,7 +19,7 @@
  * the calling thread.  Nothing unwinds across the boundary.  A context is a pool of lanes (stream + workspace each; option
  * "ctx_lanes", default 4): calls that take HOST pointers from different threads — the 15 concurrent rayon callers of
  * kimchi/src/prover.rs:329-351 — each take a free lane and overlap on the GPU; calls on an external stream, calls that take
- * device pointers and zk_srs_open (which holds the context across its callbacks) are serialised on the primary lane.
+ * device pointers, zk_srs_open and zk_srs_verify (which hold the context across their callbacks) are serialised on the primary lane.
  * There is NO CPU fallback: without a CUDA device zk_ctx_create fails with ZK_ERR_NO_DEVICE.
  */
 #ifndef ZKB200_H
@@ -272,6 +272,46 @@ int zk_srs_open(zk_srs* srs, const zk_open_poly* polys, size_t n_polys, const ui
                 const uint64_t polyscale[4], const uint64_t evalscale[4], const uint64_t* rng_scalars, size_t n_rng_scalars,
                 const zk_open_transcript* transcript, uint64_t* out_lr_xy, size_t lr_capacity_rounds, size_t* out_rounds,
                 uint64_t out_delta_xy[8], uint64_t out_z1[4], uint64_t out_z2[4], uint64_t out_sg_xy[8]);
+
+/* ------------------------------------------------------------------ SRS::verify as one call (poly-commitment/src/ipa.rs:301-502)
+ * == <OpeningProof<G> as OpenProof<G>>::verify(srs, group_map, batch, rng): batch verification of n opening proofs.  Per proof the
+ * library replays the transcript through the same three callbacks as zk_srs_open, in the reference's order — u_base(cip), then
+ * round(j, L_j, R_j) for every j, then final_challenge(delta) — proof by proof in batch order, with the context lock HELD across
+ * the callbacks (they must not call into this context).  It then checks, for all proofs at once,
+ *     0 == sum_i rand_base^i (c_i Q_i + delta_i - z1_i (G_i + b_i U_i) - z2_i H)  and  sg_i == <s_i, g>   (weighted by sg_rand_base^i)
+ * as two MSMs: one over the resident generators g with S[j] = sum_i sg_rand_base^i s_i[j] (s_i = b_poly_coefficients of the
+ * proof's challenges, built by one device kernel for the whole batch) and one over h and every proof's sg, U, L_j, R_j,
+ * commitment chunks and delta.  The challenges' inverses follow ark_ff::batch_inversion: a zero challenge stays zero.
+ *
+ * zk_verify_proof: one BatchEvaluationProof (commitment.rs:682-700) with its OpeningProof; field elements Montgomery, points
+ * affine Montgomery (identity = zeros).
+ *   lr_xy, n_rounds    n_rounds x (L, R); at most ceil(log2 |g|) rounds (more: ZK_ERR_LENGTH, the reference indexes out of bounds)
+ *   elm, n_elm         evaluation_points
+ *   comm_xy            the commitments of evaluations[..], chunk-concatenated; comm_chunks[i] chunks belong to commitment i,
+ *                      0 = an empty PolyComm (skipped without advancing the power of polyscale, commitment.rs:724-744)
+ *   transcript         this proof's sponge behind the callbacks of zk_open_transcript
+ * rng_scalars: rand_base then sg_rand_base (the reference's draw order).  *out_ok = 1 iff the batch verifies (n == 0: 1).
+ * out_sum_xyz (optional): the MSM result the reference compares with zero, Jacobian.  A callback returning non-zero or a null
+ * pointer gives ZK_ERR_INVALID.  Points are not checked to lie on the curve (the reference relies on deserialisation). */
+typedef struct zk_verify_proof {
+    const uint64_t* lr_xy;
+    size_t n_rounds;
+    const uint64_t* delta_xy;
+    const uint64_t* z1;
+    const uint64_t* z2;
+    const uint64_t* sg_xy;
+    const uint64_t* elm;
+    size_t n_elm;
+    const uint64_t* polyscale;
+    const uint64_t* evalscale;
+    const uint64_t* comm_xy;
+    const size_t* comm_chunks;
+    size_t n_comms;
+    const uint64_t* combined_inner_product;
+    const zk_open_transcript* transcript;
+} zk_verify_proof;
+int zk_srs_verify(zk_srs* srs, const zk_verify_proof* batch, size_t n, const uint64_t rng_scalars[8], int* out_ok,
+                  uint64_t out_sum_xyz[12]);
 
 /* ------------------------------------------------------------------ d8 pipeline, first pointwise evaluator (SURVEY.md §8f row 3)
  * The permutation part of the quotient polynomial in evaluation form over d8 (m = 2^log_m points), all operands resident on the

@@ -15,4 +15,6 @@ from ._lib import (  # noqa: F401
     FP, FQ, PALLAS, VESTA, BASE_FIELD, SCALAR_FIELD, ZkError, Context, Bases, lib, library_path,
     jacobian_to_affine, jacobian_sum,
 )
-from .host import SRS, ExprProgram, IndexCache, IpaRounds, OpeningProof, PolyComm, Radix2EvaluationDomain, srs_open  # noqa: F401
+from .host import (  # noqa: F401
+    SRS, BatchEvaluationProof, ExprProgram, IndexCache, IpaRounds, OpeningProof, PolyComm, Radix2EvaluationDomain, srs_open, srs_verify,
+)

@@ -124,6 +124,7 @@ def lib() -> ctypes.CDLL:
     L.zk_msm_sharded.argtypes = [vp, vp, sz, sz, vp, i, i, vp]
     L.zk_srs_open.argtypes = [vp, ctypes.POINTER(OpenPoly), sz, vp, sz, vp, vp, vp, sz, ctypes.POINTER(OpenTranscript), vp, sz,
                               ctypes.POINTER(sz), vp, vp, vp, vp]
+    L.zk_srs_verify.argtypes = [vp, ctypes.POINTER(VerifyProof), sz, vp, ctypes.POINTER(i), vp]
     return L
 
 
@@ -161,6 +162,15 @@ FINAL_CB = ctypes.CFUNCTYPE(ctypes.c_int, ctypes.c_void_p, ctypes.POINTER(ctypes
 class OpenTranscript(ctypes.Structure):
     """zk_open_transcript (include/zkb200.h)"""
     _fields_ = [("user", ctypes.c_void_p), ("u_base", U_BASE_CB), ("round", ROUND_CB), ("final_challenge", FINAL_CB)]
+
+
+class VerifyProof(ctypes.Structure):
+    """zk_verify_proof (include/zkb200.h)"""
+    _fields_ = [("lr_xy", ctypes.c_void_p), ("n_rounds", ctypes.c_size_t), ("delta_xy", ctypes.c_void_p), ("z1", ctypes.c_void_p),
+                ("z2", ctypes.c_void_p), ("sg_xy", ctypes.c_void_p), ("elm", ctypes.c_void_p), ("n_elm", ctypes.c_size_t),
+                ("polyscale", ctypes.c_void_p), ("evalscale", ctypes.c_void_p), ("comm_xy", ctypes.c_void_p),
+                ("comm_chunks", ctypes.POINTER(ctypes.c_size_t)), ("n_comms", ctypes.c_size_t), ("combined_inner_product", ctypes.c_void_p),
+                ("transcript", ctypes.POINTER(OpenTranscript))]
 
 
 def check(rc: int):

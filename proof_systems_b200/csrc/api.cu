@@ -336,6 +336,7 @@ void zk_ctx_destroy(zk_ctx* ctx) {
     if (ctx->d_scalars) cudaFree(ctx->d_scalars);
     if (ctx->d_open) cudaFree(ctx->d_open);
     if (ctx->d_ipa) cudaFree(ctx->d_ipa);
+    if (ctx->d_verify) cudaFree(ctx->d_verify);
     if (ctx->d_expr) cudaFree(ctx->d_expr);
     if (ctx->d_flag) cudaFree(ctx->d_flag);
     if (ctx->d_ntt) cudaFree(ctx->d_ntt);

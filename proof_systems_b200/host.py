@@ -245,6 +245,81 @@ def srs_open(srs, plnms, elm, polyscale, evalscale, rng_scalars, u_base, round_c
     return OpeningProof(lr[: rounds.value].copy(), delta, z1, z2, sg)
 
 
+@dataclass
+class BatchEvaluationProof:
+    """One element of the batch of SRS::verify (commitment.rs:682-700): the opening, its evaluation points and scales, the commitments
+    of `evaluations` (each uint64 [chunks, 8]; zero chunks = an empty PolyComm), the combined inner product, and the proof's own
+    transcript — the same three callables as srs_open: u_base(cip [4]) -> U [8]; round_challenge(i, l [8], r [8]) -> u [4];
+    final_challenge(delta [8]) -> c [4].  Everything in Montgomery limbs."""
+    opening: OpeningProof
+    elm: np.ndarray
+    polyscale: np.ndarray
+    evalscale: np.ndarray
+    commitments: list
+    combined_inner_product: np.ndarray
+    u_base: object
+    round_challenge: object
+    final_challenge: object
+
+
+def srs_verify(srs, batch, rand_base, sg_rand_base, return_sum: bool = False):
+    """SRS::verify (ipa.rs:301-502) through zk_srs_verify: True iff the batch of BatchEvaluationProof verifies.  rand_base and
+    sg_rand_base are the two scalars the reference draws from its rng (Montgomery [4]).  With return_sum, also the affine point [8]
+    the reference compares with zero.  An exception raised by a callback aborts the call and is re-raised here."""
+    from ._lib import FINAL_CB, ROUND_CB, U_BASE_CB, OpenTranscript, VerifyProof
+    errors, keep = [], []
+
+    def view(p, n):
+        return np.ctypeslib.as_array(p, shape=(n,)).copy()
+
+    def put(p, v, n):
+        np.ctypeslib.as_array(p, shape=(n,))[:] = np.ascontiguousarray(v, dtype=np.uint64).reshape(n)
+
+    def guard(fn):
+        def wrapped(*a):
+            try:
+                fn(*a)
+                return 0
+            except Exception as e:           # never unwind through the C frames
+                errors.append(e)
+                return 1
+        return wrapped
+
+    def arr(a, tail):
+        a = _np_u64(a, tail) if np.size(a) else np.zeros((0,) + tail, dtype=np.uint64)
+        keep.append(a)
+        return a
+
+    descs = (VerifyProof * max(1, len(batch)))()
+    for i, e in enumerate(batch):
+        op = e.opening
+        lr = arr(op.lr, (2, 8))
+        delta, sg, z1, z2 = arr(op.delta, (8,)), arr(op.sg, (8,)), arr(op.z1, (4,)), arr(op.z2, (4,))
+        elm, ps, es, cip = arr(e.elm, (4,)), arr(e.polyscale, (4,)), arr(e.evalscale, (4,)), arr(e.combined_inner_product, (4,))
+        comms = [arr(c, (8,)) for c in e.commitments]
+        cxy = arr(np.concatenate(comms) if comms else np.zeros((0, 8), dtype=np.uint64), (8,))
+        chunks = (ctypes.c_size_t * max(1, len(comms)))(*[c.shape[0] for c in comms])
+        cb = (U_BASE_CB(guard(lambda user, c, out, f=e.u_base: put(out, f(view(c, 4)), 8))),
+              ROUND_CB(guard(lambda user, j, l, r, out, f=e.round_challenge: put(out, f(int(j), view(l, 8), view(r, 8)), 4))),
+              FINAL_CB(guard(lambda user, d, out, f=e.final_challenge: put(out, f(view(d, 8)), 4))))
+        tr = OpenTranscript(None, *cb)
+        keep += [chunks, cb, tr]
+        p = lambda a: a.ctypes.data if a.size else None
+        descs[i] = VerifyProof(p(lr), lr.shape[0], p(delta), p(z1), p(z2), p(sg), p(elm), elm.shape[0], p(ps), p(es), p(cxy), chunks,
+                               len(comms), p(cip), ctypes.pointer(tr))
+    rng = np.concatenate([np.ascontiguousarray(rand_base, dtype=np.uint64).reshape(4), np.ascontiguousarray(sg_rand_base, dtype=np.uint64).reshape(4)])
+    ok = ctypes.c_int(0)
+    out = np.zeros(12, dtype=np.uint64)
+    rc = lib().zk_srs_verify(srs._h, descs, len(batch), _ptr(rng), ctypes.byref(ok), _ptr(out))
+    if errors:
+        raise errors[0]
+    check(rc)
+    if not return_sum:
+        return bool(ok.value)
+    from ._lib import jacobian_to_affine
+    return bool(ok.value), jacobian_to_affine(srs.curve, out)
+
+
 class IpaRounds:
     """The folding loop of SRS::open (poly-commitment/src/ipa.rs:929-1007) with a and b resident on the device and the bases
     taken from the resident SRS table (`bases` = ctx.upload_bases(curve, srs.g)); see csrc/ipa.cu.
