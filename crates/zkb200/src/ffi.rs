@@ -84,6 +84,22 @@ pub struct zk_expr_column {
     pub reserved: u32,
 }
 
+#[repr(C)]
+#[derive(Copy, Clone)]
+pub struct zk_eval_column {
+    pub d_evals: *const c_void,
+    pub len: u64,
+    pub boolean: u32,
+    pub reserved: u32,
+}
+
+#[repr(C)]
+#[derive(Copy, Clone)]
+pub struct zk_dev_poly {
+    pub d_coeffs: *const c_void,
+    pub len: u64,
+}
+
 extern "C" {
     pub fn zk_last_error() -> *const c_char;
     pub fn zk_ctx_create(device_id: c_int, out: *mut *mut zk_ctx) -> c_int;
@@ -123,6 +139,14 @@ extern "C" {
     pub fn zk_poly_add_dev(ctx: *mut zk_ctx, field_id: c_int, d_dst: *mut c_void, d_src: *const c_void, len: usize) -> c_int;
     pub fn zk_poly_divide_by_vanishing_dev(ctx: *mut zk_ctx, field_id: c_int, d_f: *const c_void, len: usize, log_n: c_uint,
                                            d_quot: *mut c_void, remainder_is_zero: *mut c_int) -> c_int;
+
+    pub fn zk_lagrange_evals_chunks(domain_size: usize, max_poly_size: usize) -> usize;
+    pub fn zk_lagrange_evals_dev(ctx: *mut zk_ctx, field_id: c_int, log_n: c_uint, max_poly_size: usize, x_mont: *const u64,
+                                 d_out: *mut c_void) -> c_int;
+    pub fn zk_lagrange_evaluate_dev(ctx: *mut zk_ctx, field_id: c_int, d_bases: *const *const c_void, n_points: usize, log_n: c_uint,
+                                    chunks: usize, cols: *const zk_eval_column, n_cols: usize, out: *mut u64) -> c_int;
+    pub fn zk_poly_evaluate_chunks_dev(ctx: *mut zk_ctx, field_id: c_int, polys: *const zk_dev_poly, n_polys: usize, num_chunks: usize,
+                                       chunk_size: usize, points_mont: *const u64, n_points: usize, out: *mut u64) -> c_int;
 
     pub fn zk_ntt_batch(ctx: *mut zk_ctx, field_id: c_int, data: *mut u64, log_n: c_uint, batch: usize, in_len: usize, inverse: c_int,
                         coset: c_int) -> c_int;

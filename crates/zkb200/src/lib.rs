@@ -9,10 +9,13 @@
 //!
 //! * [`expr::DeviceColumns`] runs `Expr::evaluations` (kimchi/src/circuits/expr.rs:1938-2190) — the gate and lookup constraints of
 //!   the quotient — as RPN programs over device-resident columns (`zk_expr_eval_dev`).
+//! * [`evals::DeviceLagrangeEvals`] and [`evals::evaluate_chunks_dev`] compute the prover's evaluations at zeta and zeta*omega
+//!   (kimchi/src/prover.rs:1009-1058) over the same resident columns (`zk_lagrange_evaluate_dev`, `zk_poly_evaluate_chunks_dev`).
 //!
 //! Everything called is declared in include/zkb200.h and exported by libzkb200.so; there is no CPU fallback inside the library
 //! (`Ctx::new` fails without a CUDA device) — code that must also run without a GPU keeps using `ipa::SRS`.
 pub mod domain;
+pub mod evals;
 pub mod expr;
 pub mod ffi;
 pub mod marshal;

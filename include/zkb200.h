@@ -360,6 +360,40 @@ int zk_expr_eval_dev(zk_ctx* ctx, int field_id, const zk_expr_token* tokens, siz
 int zk_poly_add_dev(zk_ctx* ctx, int field_id, void* d_dst, const void* d_src, size_t len);
 int zk_poly_divide_by_vanishing_dev(zk_ctx* ctx, int field_id, const void* d_f, size_t len, unsigned log_n, void* d_quot, int* remainder_is_zero);
 
+/* ------------------------------------------------------------------ evaluations at zeta and zeta*omega (kimchi/src/prover.rs:1009-1058)
+ * The prover's evaluation step over the columns the d8 pipeline left resident: witness, z and public coefficients (zk_ntt_dev),
+ * permutation_coefficients8 / coefficients8 / selectors (zk_index_cache_section).  Only the results cross PCIe.
+ * zk_lagrange_evals_chunks    the number of vectors of LagrangeBasisEvaluations::new(max_poly_size, D(domain_size), x): 1 if
+ *                             domain_size <= max_poly_size, else domain_size / max_poly_size; 0 when that is not a divisor (the
+ *                             reference's assert) or an argument is 0
+ * zk_lagrange_evals_dev       LagrangeBasisEvaluations::new (kimchi/src/lagrange_basis_evaluations.rs:242-258) into d_out: chunks x 2^log_n
+ *                             Montgomery elements, chunk-major.  One vector (:126-198): the normalised Lagrange basis of D(2^log_n) at
+ *                             x, all ZEROS when x lies in the domain (batch_inversion_and_mul skips the zero denominator and the
+ *                             numerator x^n - 1 is 0).  Several (:203-240): vector k is the iFFT of x^0 .. x^(m-1) at positions
+ *                             k m .. (k+1) m - 1, m = max_poly_size.  Asynchronous on the context's stream.
+ * zk_lagrange_evaluate_dev    evaluate (:72-109) / evaluate_boolean (:116-131) of n_cols resident columns against n_points bases built
+ *                             by zk_lagrange_evals_dev with the same (log_n, chunks): chunk k at point t is sum_i p[stride i] l_{t,k}[i],
+ *                             stride = len / 2^log_n; with `boolean` set, the sum of l_{t,k}[i] over every i with p[stride i] != 0 (a
+ *                             value other than 0 or 1 counts as one, like the reference).  Each column is read once for up to 8
+ *                             (point, chunk) pairs — all of them for zeta and zeta*omega with up to 4 chunks.
+ *                             out (host): n_cols x n_points x chunks x 4 u64, Montgomery.
+ * zk_poly_evaluate_chunks_dev DensePolynomial::to_chunked_polynomial(num_chunks, chunk_size).evaluate_chunks(x)
+ *                             (utils/src/dense_polynomial.rs:50-69, chunked_polynomial.rs:21-28) of n_polys resident coefficient vectors
+ *                             at n_points points (Montgomery); each vector is read once for up to 4 points.  Chunks past the end of a
+ *                             polynomial are 0.  out (host): n_polys x n_points x num_chunks x 4 u64, Montgomery.
+ * Errors, before anything runs: ZK_ERR_INVALID for a null pointer, an unknown field, log_n > 30, max_poly_size == 0, a domain larger
+ * than max_poly_size and not a multiple of it, a point that is not a canonical field element, a column length that is 0 or not a
+ * multiple of 2^log_n, a chunk count that no basis of the domain has (0, or not a divisor of 2^log_n), chunk_size == 0;
+ * ZK_ERR_LENGTH for a polynomial longer than num_chunks x chunk_size (the reference's assert_eq!). */
+size_t zk_lagrange_evals_chunks(size_t domain_size, size_t max_poly_size);
+int zk_lagrange_evals_dev(zk_ctx* ctx, int field_id, unsigned log_n, size_t max_poly_size, const uint64_t x_mont[4], void* d_out);
+typedef struct zk_eval_column { const void* d_evals; uint64_t len; uint32_t boolean; uint32_t reserved; } zk_eval_column;
+int zk_lagrange_evaluate_dev(zk_ctx* ctx, int field_id, const void* const* d_bases, size_t n_points, unsigned log_n, size_t chunks,
+                             const zk_eval_column* cols, size_t n_cols, uint64_t* out);
+typedef struct zk_dev_poly { const void* d_coeffs; uint64_t len; } zk_dev_poly;
+int zk_poly_evaluate_chunks_dev(zk_ctx* ctx, int field_id, const zk_dev_poly* polys, size_t n_polys, size_t num_chunks,
+                                size_t chunk_size, const uint64_t* points_mont, size_t n_points, uint64_t* out);
+
 /* ------------------------------------------------------------------ cached prover index (SURVEY.md §8f row 4)
  * Device-side ingestion of kimchi's mmap-backed proving-key cache, kimchi/src/cached_prover_index.rs:26-56 ("MINAPK01", format 3):
  * the file stores the index's big arrays — coefficients8 (15 columns), permutation_coefficients8 (7), the gate selectors over d4 / d8,

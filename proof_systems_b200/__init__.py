@@ -7,6 +7,7 @@ reference's interfaces on this path, with the reference's names:
     SRS.commit_non_hiding / commit_evaluations_non_hiding / mask_custom    poly-commitment/src/ipa.rs:605-728
     PolyComm                                                               poly-commitment/src/commitment.rs:47-50
     Radix2EvaluationDomain.fft_in_place / ifft_in_place                    ark_poly (kimchi/src/circuits/domains.rs:24-33)
+    LagrangeBasisEvaluations.new / evaluate / evaluate_boolean             kimchi/src/lagrange_basis_evaluations.rs:72-258
 
 There is no CPU fallback anywhere in this package: importing it without the built library, or creating a Context
 without a CUDA device, raises.
@@ -16,5 +17,5 @@ from ._lib import (  # noqa: F401
     jacobian_to_affine, jacobian_sum,
 )
 from .host import (  # noqa: F401
-    SRS, BatchEvaluationProof, ExprProgram, IndexCache, IpaRounds, OpeningProof, PolyComm, Radix2EvaluationDomain, srs_open, srs_verify,
+    SRS, BatchEvaluationProof, ExprProgram, IndexCache, IpaRounds, LagrangeBasisEvaluations, OpeningProof, PolyComm, Radix2EvaluationDomain, srs_open, srs_verify,
 )

@@ -125,6 +125,11 @@ def lib() -> ctypes.CDLL:
     L.zk_srs_open.argtypes = [vp, ctypes.POINTER(OpenPoly), sz, vp, sz, vp, vp, vp, sz, ctypes.POINTER(OpenTranscript), vp, sz,
                               ctypes.POINTER(sz), vp, vp, vp, vp]
     L.zk_srs_verify.argtypes = [vp, ctypes.POINTER(VerifyProof), sz, vp, ctypes.POINTER(i), vp]
+    L.zk_lagrange_evals_chunks.argtypes = [sz, sz]
+    L.zk_lagrange_evals_chunks.restype = sz
+    L.zk_lagrange_evals_dev.argtypes = [vp, i, u, sz, vp, vp]
+    L.zk_lagrange_evaluate_dev.argtypes = [vp, i, ctypes.POINTER(vp), sz, u, sz, ctypes.POINTER(EvalColumn), sz, vp]
+    L.zk_poly_evaluate_chunks_dev.argtypes = [vp, i, ctypes.POINTER(DevPoly), sz, sz, sz, vp, sz, vp]
     return L
 
 
@@ -145,6 +150,16 @@ class ExprToken(ctypes.Structure):
 class ExprColumn(ctypes.Structure):
     """zk_expr_column (include/zkb200.h)"""
     _fields_ = [("d_evals", ctypes.c_void_p), ("len", ctypes.c_uint64), ("domain_mult", ctypes.c_uint32), ("reserved", ctypes.c_uint32)]
+
+
+class EvalColumn(ctypes.Structure):
+    """zk_eval_column (include/zkb200.h)"""
+    _fields_ = [("d_evals", ctypes.c_void_p), ("len", ctypes.c_uint64), ("boolean", ctypes.c_uint32), ("reserved", ctypes.c_uint32)]
+
+
+class DevPoly(ctypes.Structure):
+    """zk_dev_poly (include/zkb200.h)"""
+    _fields_ = [("d_coeffs", ctypes.c_void_p), ("len", ctypes.c_uint64)]
 
 
 class OpenPoly(ctypes.Structure):
@@ -391,6 +406,38 @@ class Context:
         ok = ctypes.c_int()
         check(lib().zk_poly_divide_by_vanishing_dev(self._h, field, ctypes.c_void_p(d_f), length, log_n, ctypes.c_void_p(d_quot), ctypes.byref(ok)))
         return bool(ok.value)
+
+    # ------------------------------------------------------------------ evaluations at zeta / zeta*omega (zk_lagrange_*, zk_poly_evaluate_chunks_dev)
+    @staticmethod
+    def lagrange_evals_chunks(domain_size: int, max_poly_size: int) -> int:
+        """vectors of LagrangeBasisEvaluations::new(max_poly_size, D(domain_size), x); 0 when the reference would assert"""
+        return int(lib().zk_lagrange_evals_chunks(domain_size, max_poly_size))
+
+    def lagrange_basis_evals_dev(self, field: int, log_n: int, max_poly_size: int, x, d_out: int) -> int:
+        """zk_lagrange_evals_dev: LagrangeBasisEvaluations::new(max_poly_size, D(2^log_n), x) into d_out (chunks x 2^log_n elements,
+        chunk-major); returns the chunk count"""
+        xv = np.ascontiguousarray(x, dtype=np.uint64).reshape(4)
+        check(lib().zk_lagrange_evals_dev(self._h, field, log_n, max_poly_size, _ptr(xv), ctypes.c_void_p(d_out)))
+        return self.lagrange_evals_chunks(1 << log_n, max_poly_size)
+
+    def lagrange_evaluate_dev(self, field: int, d_bases, log_n: int, chunks: int, columns) -> np.ndarray:
+        """zk_lagrange_evaluate_dev: columns = [(device pointer, len, boolean)] against the bases d_bases (one device pointer per point,
+        built with the same log_n and chunks) -> uint64 [n_cols, n_points, chunks, 4] Montgomery"""
+        bases = (ctypes.c_void_p * max(1, len(d_bases)))(*[int(p) for p in d_bases])
+        cols = (EvalColumn * max(1, len(columns)))(*[EvalColumn(int(p), int(n), int(bool(b)), 0) for p, n, b in columns])
+        out = np.zeros((len(columns), len(d_bases), chunks, 4), dtype=np.uint64)
+        check(lib().zk_lagrange_evaluate_dev(self._h, field, bases, len(d_bases), log_n, chunks, cols, len(columns), _ptr(out)))
+        return out
+
+    def poly_evaluate_chunks_dev(self, field: int, polys, num_chunks: int, chunk_size: int, points) -> np.ndarray:
+        """zk_poly_evaluate_chunks_dev: to_chunked_polynomial(num_chunks, chunk_size).evaluate_chunks(x) of polys = [(device pointer,
+        len)] at every point of points [k, 4] (Montgomery) -> uint64 [n_polys, n_points, num_chunks, 4]"""
+        pts = np.ascontiguousarray(points, dtype=np.uint64).reshape(-1, 4)
+        arr = (DevPoly * max(1, len(polys)))(*[DevPoly(int(p), int(n)) for p, n in polys])
+        out = np.zeros((len(polys), pts.shape[0], num_chunks, 4), dtype=np.uint64)
+        check(lib().zk_poly_evaluate_chunks_dev(self._h, field, arr, len(polys), num_chunks, chunk_size, _ptr(pts) if pts.size else None,
+                                                pts.shape[0], _ptr(out)))
+        return out
 
     def points_fold_dev(self, curve: int, d_g: int, h: int, u_mont, d_out: int):
         """zk_points_fold_dev: out[i] = g[i] + [u] g[h + i] on device-resident affine points (the reference's per-round base fold)"""

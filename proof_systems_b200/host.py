@@ -413,6 +413,65 @@ class ExprProgram:
         ctx.expr_eval_dev(field, self.tokens, np.array(self.constants, dtype=np.uint64).reshape(-1, 4), cols, out_len, out_domain_mult, d_out, accumulate)
 
 
+class LagrangeBasisEvaluations:
+    """kimchi::lagrange_basis_evaluations::LagrangeBasisEvaluations (lagrange_basis_evaluations.rs:24-258) resident on the device: the
+    chunks x n basis values at x live in a device buffer this object owns (close() frees it).  Columns are (device pointer, len) pairs
+    of Montgomery evaluations whose length is a multiple of domain_size()."""
+
+    def __init__(self, ctx: Context, field: int, max_poly_size: int, log_n: int, x):
+        self.ctx, self.field, self.log_n = ctx, field, log_n
+        self.chunks = Context.lagrange_evals_chunks(1 << log_n, max_poly_size)
+        self.ptr = ctx.dev_alloc(max(1, self.chunks) << (log_n + 5))
+        try:
+            ctx.lagrange_basis_evals_dev(field, log_n, max_poly_size, x, self.ptr)
+        except Exception:
+            self.close()
+            raise
+
+    # pub fn new(max_poly_size: usize, domain: D<F>, x: F) -> LagrangeBasisEvaluations<F>
+    @classmethod
+    def new(cls, ctx: Context, field: int, max_poly_size: int, log_n: int, x) -> "LagrangeBasisEvaluations":
+        return cls(ctx, field, max_poly_size, log_n, x)
+
+    def domain_size(self) -> int:
+        return 1 << self.log_n
+
+    # pub fn evaluate<D: EvaluationDomain<F>>(&self, p: &Evaluations<F, D>) -> Vec<F>
+    def evaluate(self, column) -> np.ndarray:
+        """[chunks, 4]: chunk k is sum_i p[stride i] l_k[i]"""
+        return self.ctx.lagrange_evaluate_dev(self.field, [self.ptr], self.log_n, self.chunks, [(column[0], column[1], False)])[0, 0]
+
+    # pub fn evaluate_boolean<D: EvaluationDomain<F>>(&self, p: &Evaluations<F, D>) -> Vec<F>
+    def evaluate_boolean(self, column) -> np.ndarray:
+        """[chunks, 4]: chunk k is the sum of l_k[i] over every i with p[stride i] != 0"""
+        return self.ctx.lagrange_evaluate_dev(self.field, [self.ptr], self.log_n, self.chunks, [(column[0], column[1], True)])[0, 0]
+
+    @staticmethod
+    def evaluate_all(points, columns) -> np.ndarray:
+        """evaluate / evaluate_boolean of every column at every point in one call: points = LagrangeBasisEvaluations of one domain,
+        columns = [(device pointer, len, boolean)] -> [n_cols, n_points, chunks, 4]"""
+        p0 = points[0]
+        if any(p.log_n != p0.log_n or p.chunks != p0.chunks or p.field != p0.field for p in points):
+            raise ValueError("the bases must share field, domain and chunk count")
+        return p0.ctx.lagrange_evaluate_dev(p0.field, [p.ptr for p in points], p0.log_n, p0.chunks, columns)
+
+    def evals(self) -> np.ndarray:
+        """the basis values [chunks, n, 4] (downloaded)"""
+        return self.ctx.dev_download(self.ptr, (self.chunks, self.domain_size(), 4))
+
+    def close(self):
+        if getattr(self, "ptr", None):
+            self.ctx.dev_free(self.ptr)
+            self.ptr = None
+
+    def __del__(self):
+        try:
+            if self.ctx._h:
+                self.close()
+        except Exception:
+            pass
+
+
 class Radix2EvaluationDomain:
     """ark_poly::Radix2EvaluationDomain::<F>::new(size) on the device.  `field` is ZK_FP or ZK_FQ."""
 
