@@ -100,6 +100,14 @@ pub struct zk_dev_poly {
     pub len: u64,
 }
 
+#[repr(C)]
+#[derive(Copy, Clone)]
+pub struct zk_lin_term {
+    pub d_evals: *const c_void,
+    pub len: u64,
+    pub coeff: [u64; 4],
+}
+
 extern "C" {
     pub fn zk_last_error() -> *const c_char;
     pub fn zk_ctx_create(device_id: c_int, out: *mut *mut zk_ctx) -> c_int;
@@ -147,6 +155,9 @@ extern "C" {
                                     chunks: usize, cols: *const zk_eval_column, n_cols: usize, out: *mut u64) -> c_int;
     pub fn zk_poly_evaluate_chunks_dev(ctx: *mut zk_ctx, field_id: c_int, polys: *const zk_dev_poly, n_polys: usize, num_chunks: usize,
                                        chunk_size: usize, points_mont: *const u64, n_points: usize, out: *mut u64) -> c_int;
+    pub fn zk_prover_ft_dev(ctx: *mut zk_ctx, field_id: c_int, log_n: c_uint, max_poly_size: usize, terms: *const zk_lin_term, n_terms: usize,
+                            d_t: *const c_void, t_len: usize, zeta_mont: *const u64, d_ft: *mut c_void, ft_len: *mut usize,
+                            ft_eval1: *mut u64) -> c_int;
 
     pub fn zk_ntt_batch(ctx: *mut zk_ctx, field_id: c_int, data: *mut u64, log_n: c_uint, batch: usize, in_len: usize, inverse: c_int,
                         coset: c_int) -> c_int;

@@ -11,6 +11,8 @@
 //!   the quotient — as RPN programs over device-resident columns (`zk_expr_eval_dev`).
 //! * [`evals::DeviceLagrangeEvals`] and [`evals::evaluate_chunks_dev`] compute the prover's evaluations at zeta and zeta*omega
 //!   (kimchi/src/prover.rs:1009-1058) over the same resident columns (`zk_lagrange_evaluate_dev`, `zk_poly_evaluate_chunks_dev`).
+//! * [`ft::ft_dev`] computes the ft polynomial of Maller's optimisation (kimchi/src/prover.rs:1147-1206) from the resident quotient
+//!   and sigma_6 over d8, leaving ft resident for the opening proof (`zk_prover_ft_dev`).
 //!
 //! Everything called is declared in include/zkb200.h and exported by libzkb200.so; there is no CPU fallback inside the library
 //! (`Ctx::new` fails without a CUDA device) — code that must also run without a GPU keeps using `ipa::SRS`.
@@ -18,6 +20,7 @@ pub mod domain;
 pub mod evals;
 pub mod expr;
 pub mod ffi;
+pub mod ft;
 pub mod marshal;
 pub mod open;
 pub mod srs;

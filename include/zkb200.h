@@ -394,6 +394,23 @@ typedef struct zk_dev_poly { const void* d_coeffs; uint64_t len; } zk_dev_poly;
 int zk_poly_evaluate_chunks_dev(zk_ctx* ctx, int field_id, const zk_dev_poly* polys, size_t n_polys, size_t num_chunks,
                                 size_t chunk_size, const uint64_t* points_mont, size_t n_points, uint64_t* out);
 
+/* ------------------------------------------------------------------ ft of Maller's optimisation (kimchi/src/prover.rs:1147-1206)
+ * With n = 2^log_n, m = max_poly_size and num_chunks = 1 if n < m else n / m:
+ *     f   = interpolate(sum_k coeff_k * d_evals_k[(len_k / n) i]) over D(n)      (kimchi passes ONE term: permutation_coefficients8[6],
+ *                                                                                 8n evaluations, coefficient perm_scalar)
+ *     ft  = f.to_chunked_polynomial(num_chunks, m).linearize(zeta^m)
+ *         - t.to_chunked_polynomial(7 num_chunks, m).linearize(zeta^m).scale(zeta^n - 1)
+ * d_t: the quotient's t_len coefficients (resident; t_len = 0 is t = 0).  zeta: Montgomery, canonical; the call derives zeta^m,
+ * zeta^n and zeta * omega from it.  d_ft: room for m elements; receives all m coefficients of ft, zero past *ft_len.
+ * *ft_len: ft's length as the reference's DensePolynomial has it (one past the last nonzero coefficient; 0 for the zero polynomial).
+ * ft_eval1: ft(zeta * omega), Montgomery.  Runs on the context's stream and synchronises once.
+ * Errors, before anything runs (d_ft is untouched): ZK_ERR_INVALID for a null pointer, an unknown field, log_n > 30, max_poly_size
+ * == 0, n >= m with m not dividing n, a term whose len is not n, 2n, ..., 8n, a zeta or coefficient that is not a canonical field
+ * element; ZK_ERR_LENGTH for t longer than 7 num_chunks chunks of m (the reference's assert_eq!). */
+typedef struct zk_lin_term { const void* d_evals; uint64_t len; uint64_t coeff[4]; } zk_lin_term;
+int zk_prover_ft_dev(zk_ctx* ctx, int field_id, unsigned log_n, size_t max_poly_size, const zk_lin_term* terms, size_t n_terms,
+                     const void* d_t, size_t t_len, const uint64_t zeta_mont[4], void* d_ft, size_t* ft_len, uint64_t ft_eval1[4]);
+
 /* ------------------------------------------------------------------ cached prover index (SURVEY.md §8f row 4)
  * Device-side ingestion of kimchi's mmap-backed proving-key cache, kimchi/src/cached_prover_index.rs:26-56 ("MINAPK01", format 3):
  * the file stores the index's big arrays — coefficients8 (15 columns), permutation_coefficients8 (7), the gate selectors over d4 / d8,

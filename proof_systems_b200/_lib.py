@@ -130,6 +130,7 @@ def lib() -> ctypes.CDLL:
     L.zk_lagrange_evals_dev.argtypes = [vp, i, u, sz, vp, vp]
     L.zk_lagrange_evaluate_dev.argtypes = [vp, i, ctypes.POINTER(vp), sz, u, sz, ctypes.POINTER(EvalColumn), sz, vp]
     L.zk_poly_evaluate_chunks_dev.argtypes = [vp, i, ctypes.POINTER(DevPoly), sz, sz, sz, vp, sz, vp]
+    L.zk_prover_ft_dev.argtypes = [vp, i, u, sz, ctypes.POINTER(LinTerm), sz, vp, sz, vp, vp, ctypes.POINTER(sz), vp]
     return L
 
 
@@ -160,6 +161,11 @@ class EvalColumn(ctypes.Structure):
 class DevPoly(ctypes.Structure):
     """zk_dev_poly (include/zkb200.h)"""
     _fields_ = [("d_coeffs", ctypes.c_void_p), ("len", ctypes.c_uint64)]
+
+
+class LinTerm(ctypes.Structure):
+    """zk_lin_term (include/zkb200.h)"""
+    _fields_ = [("d_evals", ctypes.c_void_p), ("len", ctypes.c_uint64), ("coeff", ctypes.c_uint64 * 4)]
 
 
 class OpenPoly(ctypes.Structure):
@@ -438,6 +444,22 @@ class Context:
         check(lib().zk_poly_evaluate_chunks_dev(self._h, field, arr, len(polys), num_chunks, chunk_size, _ptr(pts) if pts.size else None,
                                                 pts.shape[0], _ptr(out)))
         return out
+
+    # ------------------------------------------------------------------ ft of Maller's optimisation (zk_prover_ft_dev)
+    def prover_ft_dev(self, field: int, log_n: int, max_poly_size: int, terms, d_t: int, t_len: int, zeta_mont, d_ft: int):
+        """zk_prover_ft_dev (kimchi/src/prover.rs:1147-1206): f = interpolate(sum coeff * evals[(len / n) i]) over D(2^log_n) from
+        terms = [(device pointer, len, coeff_mont)], ft = f's chunks linearised at zeta^m minus (zeta^n - 1) times t's (d_t: t_len
+        resident coefficients), written to d_ft (room for max_poly_size elements, zero past ft_len).  Returns (ft_len, ft(zeta omega)
+        as uint64 [4] Montgomery)."""
+        zv = np.ascontiguousarray(zeta_mont, dtype=np.uint64).reshape(4)
+        arr = (LinTerm * max(1, len(terms)))()
+        for k, (p, n, c) in enumerate(terms):
+            arr[k].d_evals, arr[k].len = int(p), int(n)
+            arr[k].coeff[:] = [int(v) for v in np.ascontiguousarray(c, dtype=np.uint64).reshape(4)]
+        ft_len, ev1 = ctypes.c_size_t(), np.zeros(4, dtype=np.uint64)
+        check(lib().zk_prover_ft_dev(self._h, field, log_n, max_poly_size, arr, len(terms), ctypes.c_void_p(d_t), t_len, _ptr(zv),
+                                     ctypes.c_void_p(d_ft), ctypes.byref(ft_len), _ptr(ev1)))
+        return int(ft_len.value), ev1
 
     def points_fold_dev(self, curve: int, d_g: int, h: int, u_mont, d_out: int):
         """zk_points_fold_dev: out[i] = g[i] + [u] g[h + i] on device-resident affine points (the reference's per-round base fold)"""

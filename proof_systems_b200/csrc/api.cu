@@ -339,6 +339,7 @@ void zk_ctx_destroy(zk_ctx* ctx) {
     if (ctx->d_verify) cudaFree(ctx->d_verify);
     if (ctx->d_expr) cudaFree(ctx->d_expr);
     if (ctx->d_evals) cudaFree(ctx->d_evals);
+    if (ctx->d_ft) cudaFree(ctx->d_ft);
     if (ctx->d_flag) cudaFree(ctx->d_flag);
     if (ctx->d_ntt) cudaFree(ctx->d_ntt);
     if (ctx->d_ntt_tmp) cudaFree(ctx->d_ntt_tmp);

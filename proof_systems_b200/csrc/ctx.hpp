@@ -53,6 +53,8 @@ struct zk_ctx {
     size_t cap_verify = 0;
     void* d_evals = nullptr;             // zk_lagrange_evaluate_dev / zk_poly_evaluate_chunks_dev: descriptors | partial sums | results
     size_t cap_evals = 0;
+    void* d_ft = nullptr;                // zk_prover_ft_dev: f over d1 | term descriptors | length counter
+    size_t cap_ft = 0;
     uint64_t launches = 0;
     bool profile = false;                // per-stage device timing (zk_ctx_set_profile)
     cudaEvent_t ev_ntt[2] = {nullptr, nullptr};

@@ -26,6 +26,7 @@
 
 #include "../../include/zkb200.h"
 #include "ctx.hpp"
+#include "poly.cuh"
 
 using namespace zkb;
 
@@ -251,6 +252,49 @@ template <class FS> static fe host_basis_scale(const fe& x, unsigned log_n) {
     return fe_mul<FS>(fe_sub<FS>(fe_pow_u64<FS>(x, (uint64_t)1 << log_n), fe_one<FS>()), fe_inv<FS>(fe_to_mont<FS>(n)));
 }
 
+// the chunks holding coefficients, segments per chunk and blocks per chunk of evaluate_chunks over polynomials of up to max_len
+static void chunk_plan(uint64_t max_len, size_t chunk_size, uint64_t* covered, uint64_t* spc, uint64_t* bpc) {
+    *covered = (max_len + chunk_size - 1) / chunk_size;
+    *spc = (std::min<uint64_t>(chunk_size, max_len) + HS_SEG - 1) / HS_SEG;
+    *bpc = (*spc + EV_THREADS - 1) / EV_THREADS;
+}
+
+int ctx_evaluate_chunks(zk_ctx* ctx, int field_id, const zk_dev_poly* polys, size_t n_polys, size_t chunk_size, const uint64_t* points_mont,
+                        size_t n_points, std::vector<uint8_t>& stage, const fe** d_res, uint64_t* covered_out) {
+    uint64_t max_len = 0;
+    for (size_t k = 0; k < n_polys; k++) max_len = std::max(max_len, polys[k].len);
+    uint64_t covered, spc, bpc;
+    chunk_plan(max_len, chunk_size, &covered, &spc, &bpc);
+    *covered_out = covered;
+    const size_t n_cov = n_polys * n_points * covered;
+    if (n_cov == 0) return ZK_OK;
+    cudaStream_t st = ctx->stream;
+    // context scratch: polynomial table | points | partial sums | results
+    const size_t b_pol = ((n_polys * sizeof(DevPoly)) + 255) & ~(size_t)255, b_pts = ((n_points * sizeof(fe)) + 255) & ~(size_t)255;
+    const size_t o_part = b_pol + b_pts, o_res = o_part + n_cov * bpc * sizeof(fe), total = o_res + n_cov * sizeof(fe);
+    int rc = ctx_ensure(&ctx->d_evals, &ctx->cap_evals, total);
+    if (rc) return rc;
+    stage.assign(b_pol + b_pts, 0);
+    for (size_t k = 0; k < n_polys; k++) {
+        const DevPoly d{(const fe*)polys[k].d_coeffs, polys[k].len};
+        memcpy(stage.data() + k * sizeof(DevPoly), &d, sizeof(DevPoly));
+    }
+    memcpy(stage.data() + b_pol, points_mont, n_points * sizeof(fe));
+    uint8_t* base = (uint8_t*)ctx->d_evals;
+    ZK_CUDA(cudaMemcpyAsync(base, stage.data(), stage.size(), cudaMemcpyHostToDevice, st));
+    ChunkEvalArgs a{};
+    a.polys = (const DevPoly*)base; a.points = (const fe*)(base + b_pol); a.partial = (fe*)(base + o_part);
+    a.chunk_size = chunk_size; a.n_points = (unsigned)n_points; a.covered = (unsigned)covered; a.spc = (unsigned)spc; a.bpc = (unsigned)bpc;
+    const dim3 grid((unsigned)(covered * bpc), (unsigned)n_polys, (unsigned)((n_points + HS_PTS - 1) / HS_PTS));
+    fe* res = (fe*)(base + o_res);
+    if (field_id == ZK_FP) { k_evaluate_chunks<FpParams><<<grid, EV_THREADS, 0, st>>>(a); rc = launch_sum<FpParams>(a.partial, bpc, res, n_cov, st); }
+    else { k_evaluate_chunks<FqParams><<<grid, EV_THREADS, 0, st>>>(a); rc = launch_sum<FqParams>(a.partial, bpc, res, n_cov, st); }
+    if (rc) return rc;
+    ctx->launches += 1 + (n_cov + 65534) / 65535;
+    *d_res = res;
+    return ZK_OK;
+}
+
 }  // namespace zkb
 
 extern "C" {
@@ -363,10 +407,8 @@ int zk_poly_evaluate_chunks_dev(zk_ctx* ctx, int field_id, const zk_dev_poly* po
     for (size_t t = 0; t < n_points; t++)
         if (!canonical(field_id, points_mont + 4 * t)) { zk_set_error("evaluate_chunks: point %zu is not a canonical field element", t); return ZK_ERR_INVALID; }
     uint64_t max_len = 0;
-    std::vector<DevPoly> hp(n_polys);
     for (size_t k = 0; k < n_polys; k++) {
         if (!polys[k].d_coeffs && polys[k].len) { zk_set_error("evaluate_chunks: polynomial %zu is null", k); return ZK_ERR_INVALID; }
-        hp[k] = DevPoly{(const fe*)polys[k].d_coeffs, polys[k].len};
         max_len = std::max(max_len, polys[k].len);
     }
     for (size_t k = 0; k < n_polys; k++)
@@ -377,34 +419,19 @@ int zk_poly_evaluate_chunks_dev(zk_ctx* ctx, int field_id, const zk_dev_poly* po
     const size_t n_out = n_polys * n_points * num_chunks;
     if (n_out == 0) return ZK_OK;
     memset(out, 0, n_out * sizeof(fe));                 // chunks past the end of every polynomial: the zero polynomial
-    const uint64_t covered = (max_len + chunk_size - 1) / chunk_size;
+    uint64_t covered, spc, bpc;
+    chunk_plan(max_len, chunk_size, &covered, &spc, &bpc);
     if (covered == 0) return ZK_OK;
-    const uint64_t spc = (std::min<uint64_t>(chunk_size, max_len) + HS_SEG - 1) / HS_SEG, bpc = (spc + EV_THREADS - 1) / EV_THREADS;
     if (covered * bpc > 0x7fffffffu) { zk_set_error("evaluate_chunks: %llu coefficients per polynomial are too many", (unsigned long long)max_len); return ZK_ERR_INVALID; }
     const size_t n_cov = n_polys * n_points * covered;
 
     std::lock_guard<std::mutex> lk(ctx->mu);
     ZK_CUDA(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
-    // context scratch: polynomial table | points | partial sums | results
-    const size_t b_pol = ((n_polys * sizeof(DevPoly)) + 255) & ~(size_t)255, b_pts = ((n_points * sizeof(fe)) + 255) & ~(size_t)255;
-    const size_t o_part = b_pol + b_pts, o_res = o_part + n_cov * bpc * sizeof(fe), total = o_res + n_cov * sizeof(fe);
-    int rc = ctx_ensure(&ctx->d_evals, &ctx->cap_evals, total);
+    std::vector<uint8_t> stage;
+    const fe* res = nullptr;
+    int rc = ctx_evaluate_chunks(ctx, field_id, polys, n_polys, chunk_size, points_mont, n_points, stage, &res, &covered);
     if (rc) return rc;
-    std::vector<uint8_t> stage(b_pol + b_pts, 0);
-    memcpy(stage.data(), hp.data(), n_polys * sizeof(DevPoly));
-    memcpy(stage.data() + b_pol, points_mont, n_points * sizeof(fe));
-    uint8_t* base = (uint8_t*)ctx->d_evals;
-    ZK_CUDA(cudaMemcpyAsync(base, stage.data(), stage.size(), cudaMemcpyHostToDevice, st));
-    ChunkEvalArgs a{};
-    a.polys = (const DevPoly*)base; a.points = (const fe*)(base + b_pol); a.partial = (fe*)(base + o_part);
-    a.chunk_size = chunk_size; a.n_points = (unsigned)n_points; a.covered = (unsigned)covered; a.spc = (unsigned)spc; a.bpc = (unsigned)bpc;
-    const dim3 grid((unsigned)(covered * bpc), (unsigned)n_polys, (unsigned)((n_points + HS_PTS - 1) / HS_PTS));
-    fe* res = (fe*)(base + o_res);
-    if (field_id == ZK_FP) { k_evaluate_chunks<FpParams><<<grid, EV_THREADS, 0, st>>>(a); rc = launch_sum<FpParams>(a.partial, bpc, res, n_cov, st); }
-    else { k_evaluate_chunks<FqParams><<<grid, EV_THREADS, 0, st>>>(a); rc = launch_sum<FqParams>(a.partial, bpc, res, n_cov, st); }
-    if (rc) return rc;
-    ctx->launches += 1 + (n_cov + 65534) / 65535;
     std::vector<fe> h(n_cov);
     ZK_CUDA(cudaMemcpyAsync(h.data(), res, n_cov * sizeof(fe), cudaMemcpyDeviceToHost, st));
     ZK_CUDA(cudaStreamSynchronize(st));

@@ -16,12 +16,15 @@ struct HFp {
     static constexpr uint64_t R[4] = {0x34786d38fffffffdULL, 0x992c350be41914adULL, 0xffffffffffffffffULL, 0x3fffffffffffffffULL};
     static constexpr uint64_t R2[4] = {0x8c78ecb30000000fULL, 0xd7d30dbd8b0de0e7ULL, 0x7797a99bc3c95d18ULL, 0x096d41af7b9cb714ULL};
     static constexpr uint64_t INV = 11037532056220336127ULL;
+    // 2^32-th root of unity 5^T, Montgomery form (fp.rs:24-27; field.cuh's FpParams::ROOT)
+    static constexpr uint64_t ROOT[4] = {0xa28db849bad6dbf0ULL, 0x9083cd03d3b539dfULL, 0xfba6b9ca9dc8448eULL, 0x3ec928747b89c6daULL};
 };
 struct HFq {
     static constexpr uint64_t M[4] = {0x8c46eb2100000001ULL, 0x224698fc0994a8ddULL, 0x0ULL, 0x4000000000000000ULL};
     static constexpr uint64_t R[4] = {0x5b2b3e9cfffffffdULL, 0x992c350be3420567ULL, 0xffffffffffffffffULL, 0x3fffffffffffffffULL};
     static constexpr uint64_t R2[4] = {0xfc9678ff0000000fULL, 0x67bb433d891a16e3ULL, 0x7fae231004ccf590ULL, 0x096d41af7ccfdaa9ULL};
     static constexpr uint64_t INV = 10108024940646105087ULL;
+    static constexpr uint64_t ROOT[4] = {0x218077428c9942deULL, 0xcc49578921b60494ULL, 0xac2e5d27b2efbee2ULL, 0x0b79fa897f2db056ULL};
 };
 
 struct hfe {
@@ -98,6 +101,23 @@ template <class P> inline hfe inv(const hfe& a) {
         if ((e[i / 64] >> (i % 64)) & 1) { acc = started ? mul<P>(acc, a) : a; started = true; }
     }
     return acc;
+}
+// a^e (square and multiply from the top bit; a^0 = 1)
+template <class P> inline hfe pow_u64(const hfe& a, uint64_t e) {
+    hfe acc = one<P>();
+    for (int i = 63; i >= 0; i--) {
+        acc = sqr<P>(acc);
+        if ((e >> i) & 1) acc = mul<P>(acc, a);
+    }
+    return acc;
+}
+// the generator of the 2^log_n subgroup, (5^T)^(2^(32 - log_n)) (log_n <= 32): ark's Radix2EvaluationDomain group_gen, the same
+// element the NTT tables are built from (ntt.cu)
+template <class P> inline hfe root_of_unity(unsigned log_n) {
+    hfe w;
+    memcpy(w.l, P::ROOT, 32);
+    for (unsigned i = log_n; i < 32; i++) w = sqr<P>(w);
+    return w;
 }
 
 struct hxyzz { hfe X, Y, ZZ, ZZZ; };

@@ -17,43 +17,11 @@
 #include "host_field.hpp"
 #include "ipa.hpp"
 #include "msm.cuh"
+#include "poly.cuh"
 
 using namespace zkb;
 
 namespace zkb {
-
-struct alignas(16) CombineDesc {
-    const fe* p;        // element i of the term is p[i * stride]
-    uint32_t len;       // number of elements the term contributes (i < len)
-    uint32_t stride;
-    fe scale;           // Montgomery
-};
-static_assert(sizeof(CombineDesc) == 48, "layout");
-
-// out[i] = sum_d scale_d * p_d[i * stride_d]  (i < len_d), i < n_out
-template <class FS> __global__ void k_combine(const CombineDesc* __restrict__ descs, unsigned nd, fe* out, size_t n_out) {
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_out) return;
-    fe acc = fe_zero();
-    for (unsigned d = 0; d < nd; d++) {
-        const uint32_t len = descs[d].len;
-        if (i < len) acc = fe_add<FS>(acc, fe_mul<FS>(load_fe_nc(descs[d].p + i * (size_t)descs[d].stride), load_fe_nc(&descs[d].scale)));
-    }
-    store_fe(out + i, acc);
-}
-
-// a[i] += sum_k zeta^k * e[k * chunk + i]   (to_chunked_polynomial(num_chunks, chunk).linearize(polyscale), utils.rs:190-199)
-template <class FS> __global__ void k_linearize_add(fe* a, const fe* __restrict__ e, size_t e_len, size_t chunk, unsigned num_chunks, fe zeta) {
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= chunk) return;
-    fe acc = load_fe(a + i), scale = fe_one<FS>();
-    for (unsigned k = 0; k < num_chunks; k++) {
-        const size_t j = (size_t)k * chunk + i;
-        if (j < e_len) acc = fe_add<FS>(acc, fe_mul<FS>(load_fe_nc(e + j), scale));
-        scale = fe_mul<FS>(scale, zeta);
-    }
-    store_fe(a + i, acc);
-}
 
 // b[j] = sum_i scale_i * elm_i^j   (ipa.rs:876-888; pows(padded_length, e))
 template <class FS> __global__ void k_b_init(const fe* __restrict__ elm, const fe* __restrict__ scales, unsigned n_elm, fe* b, size_t n) {
@@ -227,7 +195,7 @@ static int open_impl(zk_srs* srs, const zk_open_poly* polys, size_t n_polys, con
         const unsigned num_chunks = (unsigned)((degree + srs_len - 1) / srs_len);
         fe zeta;
         memcpy(&zeta, polyscale, 32);
-        k_linearize_add<FS><<<(unsigned)((srs_len + 127) / 128), 128, 0, st>>>(s->d_a, d_evals, degree, srs_len, num_chunks, zeta);
+        k_linearize_add<FS><<<(unsigned)((srs_len + 127) / 128), 128, 0, st>>>(s->d_a, d_evals, degree, srs_len, num_chunks, zeta, fe_one<FS>());
         ctx->launches += 2;
     }
     // ---- b_init and the combined inner product (ipa.rs:876-896)
