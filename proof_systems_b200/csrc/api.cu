@@ -7,7 +7,6 @@
 
 #include "../../include/zkb200.h"
 #include "ctx.hpp"
-#include "host_field.hpp"
 #include "msm.cuh"
 #include "ntt.cuh"
 #include "quad.cuh"
@@ -47,7 +46,7 @@ template <class HP> static host::hxyzz msm_finish_t(const xyzz_t* T, unsigned c,
 }
 
 static void xyzz_to_jac_out(int curve, const host::hxyzz& p, uint64_t out[12]) {
-    host::hjac j = curve == ZK_PALLAS ? host::to_jacobian<host::HFp>(p) : host::to_jacobian<host::HFq>(p);
+    const host::hjac j = with_curve(curve, [&](auto c) { return host::to_jacobian<typename decltype(c)::HP>(p); });
     memcpy(out, &j, sizeof j);
 }
 
@@ -60,7 +59,6 @@ int ctx_msm_many(zk_ctx* ctx, const zk_bases* bases, size_t off, size_t n, const
 int ctx_msm_many_offs(zk_ctx* ctx, const zk_bases* bases, const size_t* offs, size_t n, const fe* const* d_scalars, size_t k, int mont, int window_bits,
                       uint64_t* out_xyz, const affine_t* d_extra, size_t n_extra) {
     if (window_bits < 0 || window_bits > (int)MSM_MAX_WINDOW_BITS) { zk_set_error("msm: window_bits %d outside [0, %u]", window_bits, MSM_MAX_WINDOW_BITS); return ZK_ERR_INVALID; }
-    const bool pallas = bases->b.curve == ZK_PALLAS;
     // MSMs per pipeline: the context's limit, and no more than keeps the sorted entry list below 2^28 entries (1 GiB of scratch)
     const unsigned c_eff = bases->b.c ? bases->b.c : (window_bits ? (unsigned)window_bits : (unsigned)msm_default_window(n, false));
     const size_t per_msm = std::max<size_t>(1, (n + n_extra) * msm_num_windows(std::max(2u, c_eff)));
@@ -71,20 +69,20 @@ int ctx_msm_many_offs(zk_ctx* ctx, const zk_bases* bases, const size_t* offs, si
         MsmResultShape shape;
         unsigned nl = 0;
         ctx->ws.h_slot = 0;
-        int rc = pallas ? msm_run<FpParams, FqParams>(bases->b, offs + j0, n, d_scalars + j0, cnt, mont != 0, (unsigned)window_bits, ctx->ws, ctx->stream, &shape, &nl,
-                                                      d_extra, n_extra)
-                        : msm_run<FqParams, FpParams>(bases->b, offs + j0, n, d_scalars + j0, cnt, mont != 0, (unsigned)window_bits, ctx->ws, ctx->stream, &shape, &nl,
-                                                      d_extra, n_extra);
-        if (rc) return rc;
-        ctx->launches += nl;
-        for (unsigned j = 0; j < cnt; j++) {
-            host::hxyzz r = host::identity();
-            if (shape.groups) {
-                const xyzz_t* h = ctx->ws.h_bitsums + (size_t)j * shape.groups * shape.c;
-                r = pallas ? msm_finish_t<host::HFp>(h, shape.c, shape.groups) : msm_finish_t<host::HFq>(h, shape.c, shape.groups);
+        const int rc = with_curve(bases->b.curve, [&](auto c) {
+            using C = decltype(c);
+            if (int e = msm_run<typename C::F, typename C::FS>(bases->b, offs + j0, n, d_scalars + j0, cnt, mont != 0, (unsigned)window_bits, ctx->ws,
+                                                               ctx->stream, &shape, &nl, d_extra, n_extra))
+                return e;
+            ctx->launches += nl;
+            for (unsigned j = 0; j < cnt; j++) {
+                host::hxyzz r = host::identity();
+                if (shape.groups) r = msm_finish_t<typename C::HP>(ctx->ws.h_bitsums + (size_t)j * shape.groups * shape.c, shape.c, shape.groups);
+                xyzz_to_jac_out(bases->b.curve, r, out_xyz + 12 * (j0 + j));
             }
-            xyzz_to_jac_out(bases->b.curve, r, out_xyz + 12 * (j0 + j));
-        }
+            return ZK_OK;
+        });
+        if (rc) return rc;
     }
     return ZK_OK;
 }
@@ -101,23 +99,13 @@ static int ctx_side_streams_init(zk_ctx* ctx) {
     return ZK_OK;
 }
 
-int ctx_ensure(void** p, size_t* cap, size_t bytes) {
-    if (*cap >= bytes) return ZK_OK;
-    if (*p) cudaFree(*p);
-    *p = nullptr;
-    *cap = 0;
-    ZK_CUDA(cudaMalloc(p, bytes));
-    *cap = bytes;
-    return ZK_OK;
-}
-
 static int ctx_ntt_tables(zk_ctx* lane, int field, unsigned log_n, bool inverse, const fe** small, const NttTables** tabs) {
     zk_ctx* ctx = ctx_root(lane);                      // one cache per pool; entries are immutable once built
     std::lock_guard<std::mutex> tl(ctx->tab_mu);
     fe*& sm = ctx->ntt_small[field][inverse ? 1 : 0];
     if (!sm) {
         ZK_CUDA(cudaMalloc(&sm, 512 * sizeof(fe)));
-        int rc = field == ZK_FP ? ntt_build_small_table<FpParams>(sm, inverse, lane->stream) : ntt_build_small_table<FqParams>(sm, inverse, lane->stream);
+        int rc = with_field(field, [&](auto f) { return ntt_build_small_table<typename decltype(f)::Dev>(sm, inverse, lane->stream); });
         if (rc) return rc;
         lane->launches += 2;
     }
@@ -125,7 +113,7 @@ static int ctx_ntt_tables(zk_ctx* lane, int field, unsigned log_n, bool inverse,
     auto it = ctx->ntt_tables.find(key);
     if (it == ctx->ntt_tables.end()) {
         NttTables t;
-        int rc = field == ZK_FP ? ntt_build_tables<FpParams>(t, log_n, inverse, lane->stream) : ntt_build_tables<FqParams>(t, log_n, inverse, lane->stream);
+        int rc = with_field(field, [&](auto f) { return ntt_build_tables<typename decltype(f)::Dev>(t, log_n, inverse, lane->stream); });
         if (rc) return rc;
         lane->launches += t.full ? 8 : 7;
         it = ctx->ntt_tables.emplace(key, t).first;
@@ -135,7 +123,6 @@ static int ctx_ntt_tables(zk_ctx* lane, int field, unsigned log_n, bool inverse,
     return ZK_OK;
 }
 
-// the unscaled twiddle tables of a forward / inverse transform (pointwise evaluators take x_i = w^i from them)
 int ctx_ntt_table_ptrs(zk_ctx* ctx, int field, unsigned log_n, bool inverse, const fe** ulo, const fe** mid, const fe** hi2) {
     const fe* small;
     const NttTables* tabs;
@@ -148,7 +135,7 @@ int ctx_ntt_table_ptrs(zk_ctx* ctx, int field, unsigned log_n, bool inverse, con
 // Transform of `batch` polynomials: polynomial b is read from d_in + b * in_bs (its first in_len elements) and written to
 // d_out + b * 2^log_n; d_in == d_out (in_bs = 2^log_n) is the in-place form.
 int ctx_ntt_device_oop(zk_ctx* ctx, int field, const fe* d_in, size_t in_bs, fe* d_out, unsigned log_n, size_t batch, size_t in_len, int inverse, int coset) {
-    if (field != ZK_FP && field != ZK_FQ) { zk_set_error("ntt: unknown field_id %d", field); return ZK_ERR_INVALID; }
+    if (int rc = check_field("ntt", field)) return rc;
     if (log_n > NTT_MAX_LOG_N) { zk_set_error("ntt: log_n %u > %u not supported", log_n, NTT_MAX_LOG_N); return ZK_ERR_INVALID; }
     const fe* small;
     const NttTables* tabs;
@@ -163,17 +150,18 @@ int ctx_ntt_device_oop(zk_ctx* ctx, int field, const fe* d_in, size_t in_bs, fe*
     size_t bytes = ((size_t)batch << log_n) * sizeof(fe);
     fe* tmp = nullptr;
     if (log_n > NTT_MAX_LOG_SUB) {
-        rc = ctx_ensure((void**)&ctx->d_ntt_tmp, &ctx->cap_ntt_tmp, bytes);
+        rc = ctx->d_ntt_tmp.ensure(bytes);
         if (rc) return rc;
-        tmp = ctx->d_ntt_tmp;
+        tmp = ctx->d_ntt_tmp.at<fe>();
     }
     unsigned nl = 0;
     if (ctx->profile) {
         if (!ctx->ev_ntt[0]) { ZK_CUDA(cudaEventCreate(&ctx->ev_ntt[0])); ZK_CUDA(cudaEventCreate(&ctx->ev_ntt[1])); }
         ZK_CUDA(cudaEventRecord(ctx->ev_ntt[0], ctx->stream));
     }
-    rc = field == ZK_FP ? ntt_run<FpParams>(d_in, in_bs, d_out, tmp, small, *tabs, inner, log_n, batch, in_len, inverse != 0, coset != 0, ctx->stream, &nl)
-                        : ntt_run<FqParams>(d_in, in_bs, d_out, tmp, small, *tabs, inner, log_n, batch, in_len, inverse != 0, coset != 0, ctx->stream, &nl);
+    rc = with_field(field, [&](auto f) {
+        return ntt_run<typename decltype(f)::Dev>(d_in, in_bs, d_out, tmp, small, *tabs, inner, log_n, batch, in_len, inverse != 0, coset != 0, ctx->stream, &nl);
+    });
     ctx->launches += nl;
     if (rc == ZK_OK && ctx->profile) {
         ZK_CUDA(cudaEventRecord(ctx->ev_ntt[1], ctx->stream));
@@ -330,24 +318,11 @@ void zk_ctx_destroy(zk_ctx* ctx) {
     for (int l = 0; l < zk_ctx::SIDE_STREAMS; l++)
         if (ctx->side[l]) { cudaStreamSynchronize(ctx->side[l]); cudaStreamDestroy(ctx->side[l]); }
     if (ctx->ev_fork) cudaEventDestroy(ctx->ev_fork);
-    if (ctx->h_scratch) cudaFreeHost(ctx->h_scratch);
-    if (ctx->h_gather) cudaFreeHost(ctx->h_gather);
-    if (ctx->d_gather_sum) cudaFree(ctx->d_gather_sum);
-    if (ctx->d_scalars) cudaFree(ctx->d_scalars);
-    if (ctx->d_open) cudaFree(ctx->d_open);
-    if (ctx->d_ipa) cudaFree(ctx->d_ipa);
-    if (ctx->d_verify) cudaFree(ctx->d_verify);
-    if (ctx->d_expr) cudaFree(ctx->d_expr);
-    if (ctx->d_evals) cudaFree(ctx->d_evals);
-    if (ctx->d_ft) cudaFree(ctx->d_ft);
-    if (ctx->d_flag) cudaFree(ctx->d_flag);
-    if (ctx->d_ntt) cudaFree(ctx->d_ntt);
-    if (ctx->d_ntt_tmp) cudaFree(ctx->d_ntt_tmp);
     for (int f = 0; f < 2; f++) for (int d = 0; d < 2; d++) if (ctx->ntt_small[f][d]) cudaFree(ctx->ntt_small[f][d]);
     for (auto& kv : ctx->ntt_tables) ntt_free_tables(kv.second);
     for (auto& e : ctx->ev_ntt) if (e) cudaEventDestroy(e);
     cudaStreamDestroy(ctx->own_stream);
-    delete ctx;
+    delete ctx;                          // frees the scratch members on this device
 }
 
 int zk_ctx_set_stream(zk_ctx* ctx, void* cuda_stream) {
@@ -419,7 +394,7 @@ int zk_ctx_last_stage_ms(const zk_ctx* ctx, float* out, size_t capacity) {
 // ---------------------------------------------------------------------------------------------- bases
 int zk_bases_upload(zk_ctx* ctx, int curve_id, const uint64_t* xy_mont, size_t n, int window_bits, int points_on_device, zk_bases** out) {
     if (!ctx || !out || (!xy_mont && n)) { zk_set_error("bases_upload: null argument"); return ZK_ERR_INVALID; }
-    if (curve_id != ZK_PALLAS && curve_id != ZK_VESTA) { zk_set_error("bases_upload: unknown curve_id %d", curve_id); return ZK_ERR_INVALID; }
+    if (int rc = check_curve("bases_upload", curve_id)) return rc;
     if (window_bits < -1 || window_bits == 1 || window_bits > (int)MSM_MAX_WINDOW_BITS) { zk_set_error("bases_upload: window_bits %d not in {-1, 0, 2..%u}", window_bits, MSM_MAX_WINDOW_BITS); return ZK_ERR_INVALID; }
     std::lock_guard<std::mutex> lk(ctx->mu);
     ZK_CUDA(cudaSetDevice(ctx->device));
@@ -427,8 +402,7 @@ int zk_bases_upload(zk_ctx* ctx, int curve_id, const uint64_t* xy_mont, size_t n
     zk_bases* bs = new zk_bases();
     bs->ctx = ctx;
     bs->b.curve = curve_id;
-    int rc = curve_id == ZK_PALLAS ? msm_bases_create<FpParams>(bs->b, (const affine_t*)xy_mont, points_on_device != 0, n, c, ctx->stream)
-                                   : msm_bases_create<FqParams>(bs->b, (const affine_t*)xy_mont, points_on_device != 0, n, c, ctx->stream);
+    int rc = with_curve(curve_id, [&](auto cv) { return msm_bases_create<typename decltype(cv)::F>(bs->b, (const affine_t*)xy_mont, points_on_device != 0, n, c, ctx->stream); });
     if (rc) { msm_bases_free(bs->b); delete bs; return rc; }
     if (c) ctx->launches += 1;
     *out = bs;
@@ -452,45 +426,33 @@ int zk_bases_window_bits(const zk_bases* bases) { return bases ? (int)bases->b.c
 //   mode 2: affine -> 33-byte compressed
 static int points_codec(zk_ctx* ctx, int curve_id, int mode, const void* in, size_t n, void* out, const char* what) {
     if (!ctx || (!in && n) || (!out && n)) { zk_set_error("%s: null argument", what); return ZK_ERR_INVALID; }
-    if (curve_id != ZK_PALLAS && curve_id != ZK_VESTA) { zk_set_error("%s: unknown curve_id %d", what, curve_id); return ZK_ERR_INVALID; }
+    if (int rc = check_curve(what, curve_id)) return rc;
     std::lock_guard<std::mutex> lk(ctx->mu);
     ZK_CUDA(cudaSetDevice(ctx->device));
     if (n == 0) return ZK_OK;
     const size_t in_bytes = (mode == 0 ? 33 : mode == 1 ? 65 : sizeof(affine_t)) * n, out_bytes = (mode == 2 ? 33 : sizeof(affine_t)) * n;
-    void *d_in = nullptr, *d_out = nullptr;
-    unsigned* d_bad = nullptr;
+    DevScratch d_in, d_out, d_bad;       // transient: freed on every return
+    int rc = d_in.ensure(in_bytes);
+    if (rc || (rc = d_out.ensure(out_bytes)) || (rc = d_bad.ensure(sizeof(unsigned)))) return rc;
+    ZK_CUDA(cudaMemsetAsync(d_bad.p, 0, sizeof(unsigned), ctx->stream));
+    ZK_CUDA(cudaMemcpyAsync(d_in.p, in, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    rc = with_curve(curve_id, [&](auto c) {
+        using F = typename decltype(c)::F;
+        if (mode == 0) return points_decompress<F>(d_in.at<uint8_t>(), d_out.at<affine_t>(), n, d_bad.at<unsigned>(), ctx->stream);
+        if (mode == 1) return points_from_uncompressed<F>(d_in.at<uint8_t>(), d_out.at<affine_t>(), n, d_bad.at<unsigned>(), ctx->stream);
+        return points_compress<F>(d_in.at<affine_t>(), d_out.at<uint8_t>(), n, ctx->stream);
+    });
+    if (rc) return rc;
+    ctx->launches += 1;
     unsigned bad = 0;
-    cudaError_t e = cudaMalloc(&d_in, in_bytes);
-    if (e == cudaSuccess) e = cudaMalloc(&d_out, out_bytes);
-    if (e == cudaSuccess) e = cudaMalloc(&d_bad, sizeof(unsigned));
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_bad, 0, sizeof(unsigned), ctx->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_in, in, in_bytes, cudaMemcpyHostToDevice, ctx->stream);
-    int rc = ZK_OK;
-    if (e == cudaSuccess) {
-        const bool pallas = curve_id == ZK_PALLAS;
-        if (mode == 0)
-            rc = pallas ? points_decompress<FpParams>((const uint8_t*)d_in, (affine_t*)d_out, n, d_bad, ctx->stream)
-                        : points_decompress<FqParams>((const uint8_t*)d_in, (affine_t*)d_out, n, d_bad, ctx->stream);
-        else if (mode == 1)
-            rc = pallas ? points_from_uncompressed<FpParams>((const uint8_t*)d_in, (affine_t*)d_out, n, d_bad, ctx->stream)
-                        : points_from_uncompressed<FqParams>((const uint8_t*)d_in, (affine_t*)d_out, n, d_bad, ctx->stream);
-        else
-            rc = pallas ? points_compress<FpParams>((const affine_t*)d_in, (uint8_t*)d_out, n, ctx->stream)
-                        : points_compress<FqParams>((const affine_t*)d_in, (uint8_t*)d_out, n, ctx->stream);
-        if (rc == ZK_OK) {
-            ctx->launches += 1;
-            e = cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, ctx->stream);
-            if (e == cudaSuccess) e = cudaMemcpyAsync(&bad, d_bad, sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream);
-            if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-        }
-    }
-    cudaFree(d_in); cudaFree(d_out); cudaFree(d_bad);
-    if (e != cudaSuccess) { zk_set_error("%s: %s", what, cudaGetErrorString(e)); return ZK_ERR_CUDA; }
-    if (rc == ZK_OK && bad) {
+    ZK_CUDA(cudaMemcpyAsync(out, d_out.p, out_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    ZK_CUDA(cudaMemcpyAsync(&bad, d_bad.p, sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));
+    ZK_CUDA(cudaStreamSynchronize(ctx->stream));
+    if (bad) {
         zk_set_error(mode == 0 ? "%s: %u of %zu encodings are invalid (x off the curve, x >= modulus, or unknown flag bits)" : "%s: %u of %zu points have a non-canonical coordinate", what, bad, n);
         return ZK_ERR_INVALID;
     }
-    return rc;
+    return ZK_OK;
 }
 
 int zk_points_decompress(zk_ctx* ctx, int curve_id, const uint8_t* in33, size_t n, uint64_t* out_xy) {
@@ -505,22 +467,18 @@ int zk_points_compress(zk_ctx* ctx, int curve_id, const uint64_t* xy_mont, size_
 
 int zk_points_synthetic(zk_ctx* ctx, int curve_id, uint64_t seed, size_t n, uint64_t* out_xy) {
     if (!ctx || (!out_xy && n)) { zk_set_error("points_synthetic: null argument"); return ZK_ERR_INVALID; }
-    if (curve_id != ZK_PALLAS && curve_id != ZK_VESTA) { zk_set_error("points_synthetic: unknown curve_id %d", curve_id); return ZK_ERR_INVALID; }
+    if (int rc = check_curve("points_synthetic", curve_id)) return rc;
     std::lock_guard<std::mutex> lk(ctx->mu);
     ZK_CUDA(cudaSetDevice(ctx->device));
     if (n == 0) return ZK_OK;
-    affine_t* d = nullptr;
-    ZK_CUDA(cudaMalloc(&d, n * sizeof(affine_t)));
-    int rc = curve_id == ZK_PALLAS ? points_synthetic<FpParams>(d, n, seed, ctx->stream) : points_synthetic<FqParams>(d, n, seed, ctx->stream);
-    cudaError_t e = cudaSuccess;
-    if (rc == ZK_OK) {
-        ctx->launches += 1;
-        e = cudaMemcpyAsync(out_xy, d, n * sizeof(affine_t), cudaMemcpyDeviceToHost, ctx->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    }
-    cudaFree(d);
-    if (e != cudaSuccess) { zk_set_error("points_synthetic: %s", cudaGetErrorString(e)); return ZK_ERR_CUDA; }
-    return rc;
+    DevScratch d;                        // transient: freed on every return
+    if (int rc = d.ensure(n * sizeof(affine_t))) return rc;
+    int rc = with_curve(curve_id, [&](auto c) { return points_synthetic<typename decltype(c)::F>(d.at<affine_t>(), n, seed, ctx->stream); });
+    if (rc) return rc;
+    ctx->launches += 1;
+    ZK_CUDA(cudaMemcpyAsync(out_xy, d.p, n * sizeof(affine_t), cudaMemcpyDeviceToHost, ctx->stream));
+    ZK_CUDA(cudaStreamSynchronize(ctx->stream));
+    return ZK_OK;
 }
 
 // ---------------------------------------------------------------------------------------------- MSM
@@ -549,10 +507,10 @@ int zk_msm_batch(zk_ctx* root, const zk_bases* bases, size_t off, size_t n, cons
         d_sc = (const fe*)attr.devicePointer;
     } else {
         cudaGetLastError();  // clear the "invalid value" some drivers report for pageable pointers
-        rc = ctx_ensure((void**)&ctx->d_scalars, &ctx->cap_scalars, std::max<size_t>(k * n, 1) * sizeof(fe));
+        rc = ctx->d_scalars.ensure(std::max<size_t>(k * n, 1) * sizeof(fe));
         if (rc) return rc;
-        if (n) ZK_CUDA(cudaMemcpyAsync(ctx->d_scalars, scalars, k * n * sizeof(fe), cudaMemcpyHostToDevice, ctx->stream));
-        d_sc = ctx->d_scalars;
+        d_sc = ctx->d_scalars.at<fe>();
+        if (n) ZK_CUDA(cudaMemcpyAsync(ctx->d_scalars.p, scalars, k * n * sizeof(fe), cudaMemcpyHostToDevice, ctx->stream));
     }
     std::vector<const fe*> scs(k);
     for (size_t j = 0; j < k; j++) scs[j] = d_sc + j * n;
@@ -576,18 +534,18 @@ static int msm_partial_impl(zk_ctx* ctx, const zk_bases* bases, size_t off, size
     } else if (known && attr.type == cudaMemoryTypeHost && attr.devicePointer) {
         d_sc = (const fe*)attr.devicePointer;          // page-locked: read over PCIe by the recode kernel
     } else {
-        int rc = ctx_ensure((void**)&ctx->d_scalars, &ctx->cap_scalars, n * sizeof(fe));
-        if (rc) return rc;
-        ZK_CUDA(cudaMemcpyAsync(ctx->d_scalars, scalars, n * sizeof(fe), cudaMemcpyHostToDevice, ctx->stream));
-        d_sc = ctx->d_scalars;
+        if (int rc = ctx->d_scalars.ensure(n * sizeof(fe))) return rc;
+        d_sc = ctx->d_scalars.at<fe>();
+        ZK_CUDA(cudaMemcpyAsync(ctx->d_scalars.p, scalars, n * sizeof(fe), cudaMemcpyHostToDevice, ctx->stream));
     }
     MsmResultShape shape;
     unsigned nl = 0;
     ctx->ws.d_T_out = (xyzz_t*)d_out;
     ctx->ws.d_T_cap = capacity_points;
-    int rc = bases->b.curve == ZK_PALLAS
-                 ? msm_run<FpParams, FqParams>(bases->b, &off, n, &d_sc, 1, scalars_are_mont != 0, (unsigned)window_bits, ctx->ws, ctx->stream, &shape, &nl)
-                 : msm_run<FqParams, FpParams>(bases->b, &off, n, &d_sc, 1, scalars_are_mont != 0, (unsigned)window_bits, ctx->ws, ctx->stream, &shape, &nl);
+    int rc = with_curve(bases->b.curve, [&](auto c) {
+        using C = decltype(c);
+        return msm_run<typename C::F, typename C::FS>(bases->b, &off, n, &d_sc, 1, scalars_are_mont != 0, (unsigned)window_bits, ctx->ws, ctx->stream, &shape, &nl);
+    });
     ctx->ws.d_T_out = nullptr;
     ctx->ws.d_T_cap = 0;
     ctx->launches += nl;
@@ -601,26 +559,21 @@ static int msm_partial_impl(zk_ctx* ctx, const zk_bases* bases, size_t off, size
 // per slice on the device, copies groups*c points to the host and finishes the O(c) tail there.
 static int msm_finish_gathered_impl(zk_ctx* ctx, int curve_id, const void* d_all, size_t world, unsigned c, unsigned groups, uint64_t out_xyz[12]) {
     if (!ctx || !d_all || !out_xyz || world == 0) { zk_set_error("msm_finish_gathered: null argument"); return ZK_ERR_INVALID; }
-    if (curve_id != ZK_PALLAS && curve_id != ZK_VESTA) { zk_set_error("msm_finish_gathered: unknown curve_id %d", curve_id); return ZK_ERR_INVALID; }
+    if (int rc = check_curve("msm_finish_gathered", curve_id)) return rc;
     const size_t count = (size_t)c * groups;
     if (count == 0 || count > 4096) { zk_set_error("msm_finish_gathered: bad shape c = %u, groups = %u", c, groups); return ZK_ERR_INVALID; }
-    int rc = ctx_ensure((void**)&ctx->d_gather_sum, &ctx->cap_gather_sum, count * sizeof(xyzz_t));
-    if (rc) return rc;
-    if (ctx->cap_h_gather < count) {
-        if (ctx->h_gather) cudaFreeHost(ctx->h_gather);
-        ctx->h_gather = nullptr; ctx->cap_h_gather = 0;
-        ZK_CUDA(cudaMallocHost(&ctx->h_gather, count * sizeof(xyzz_t)));
-        ctx->cap_h_gather = count;
-    }
-    rc = curve_id == ZK_PALLAS ? msm_sum_partials<FpParams>((const xyzz_t*)d_all, world, count, ctx->d_gather_sum, ctx->stream)
-                               : msm_sum_partials<FqParams>((const xyzz_t*)d_all, world, count, ctx->d_gather_sum, ctx->stream);
-    if (rc) return rc;
-    ctx->launches += 1;
-    ZK_CUDA(cudaMemcpyAsync(ctx->h_gather, ctx->d_gather_sum, count * sizeof(xyzz_t), cudaMemcpyDeviceToHost, ctx->stream));
-    ZK_CUDA(cudaStreamSynchronize(ctx->stream));
-    host::hxyzz r = curve_id == ZK_PALLAS ? msm_finish_t<host::HFp>(ctx->h_gather, c, groups) : msm_finish_t<host::HFq>(ctx->h_gather, c, groups);
-    xyzz_to_jac_out(curve_id, r, out_xyz);
-    return ZK_OK;
+    if (int rc = ctx->d_gather_sum.ensure(count * sizeof(xyzz_t))) return rc;
+    if (int rc = ctx->h_gather.ensure(count * sizeof(xyzz_t))) return rc;
+    xyzz_t *d_sum = ctx->d_gather_sum.at<xyzz_t>(), *h_sum = ctx->h_gather.at<xyzz_t>();
+    return with_curve(curve_id, [&](auto cv) {
+        using C = decltype(cv);
+        if (int e = msm_sum_partials<typename C::F>((const xyzz_t*)d_all, world, count, d_sum, ctx->stream)) return e;
+        ctx->launches += 1;
+        ZK_CUDA(cudaMemcpyAsync(h_sum, d_sum, count * sizeof(xyzz_t), cudaMemcpyDeviceToHost, ctx->stream));
+        ZK_CUDA(cudaStreamSynchronize(ctx->stream));
+        xyzz_to_jac_out(curve_id, msm_finish_t<typename C::HP>(h_sum, c, groups), out_xyz);
+        return ZK_OK;
+    });
 }
 
 int zk_msm_partial(zk_ctx* ctx, const zk_bases* bases, size_t off, size_t n, const void* scalars, int scalars_are_mont, int window_bits,
@@ -641,31 +594,24 @@ int zk_msm(zk_ctx* ctx, const zk_bases* bases, size_t off, size_t n, const uint6
     return zk_msm_batch(ctx, bases, off, n, scalars, 1, scalars_are_mont, window_bits, out_xyz);
 }
 
-static int check_curve(int curve_id) {
-    if (curve_id != ZK_PALLAS && curve_id != ZK_VESTA) { zk_set_error("unknown curve_id %d", curve_id); return ZK_ERR_INVALID; }
-    return ZK_OK;
-}
-
 int zk_jacobian_to_affine(int curve_id, const uint64_t xyz[12], uint64_t out_xy[8]) {
     if (!xyz || !out_xy) { zk_set_error("null argument"); return ZK_ERR_INVALID; }
-    if (int rc = check_curve(curve_id)) return rc;
+    if (int rc = check_curve(nullptr, curve_id)) return rc;
     host::hjac j;
     memcpy(&j, xyz, sizeof j);
-    host::haffine a = curve_id == ZK_PALLAS ? host::to_affine<host::HFp>(host::from_jacobian<host::HFp>(j))
-                                            : host::to_affine<host::HFq>(host::from_jacobian<host::HFq>(j));
+    const host::haffine a = with_curve(curve_id, [&](auto c) { using HP = typename decltype(c)::HP; return host::to_affine<HP>(host::from_jacobian<HP>(j)); });
     memcpy(out_xy, &a, sizeof a);
     return ZK_OK;
 }
 
 int zk_jacobian_sum(int curve_id, const uint64_t* xyz, size_t count, uint64_t out_xyz[12]) {
     if ((!xyz && count) || !out_xyz) { zk_set_error("null argument"); return ZK_ERR_INVALID; }
-    if (int rc = check_curve(curve_id)) return rc;
+    if (int rc = check_curve(nullptr, curve_id)) return rc;
     host::hxyzz acc = host::identity();
     for (size_t i = 0; i < count; i++) {
         host::hjac j;
         memcpy(&j, xyz + 12 * i, sizeof j);
-        acc = curve_id == ZK_PALLAS ? host::padd<host::HFp>(acc, host::from_jacobian<host::HFp>(j))
-                                    : host::padd<host::HFq>(acc, host::from_jacobian<host::HFq>(j));
+        acc = with_curve(curve_id, [&](auto c) { using HP = typename decltype(c)::HP; return host::padd<HP>(acc, host::from_jacobian<HP>(j)); });
     }
     xyzz_to_jac_out(curve_id, acc, out_xyz);
     return ZK_OK;
@@ -746,8 +692,9 @@ int zk_ntt_batch(zk_ctx* root, int field_id, uint64_t* data, unsigned log_n, siz
     if (in_len == 0 || in_len > n || inverse) in_len = n;
     // (Transforming page-locked memory in place over PCIe was measured and is slower than two staged copies: the tile loads
     //  are 64-128 B requests.  MSM scalars, read once in full lines, do take the zero-copy route — zk_msm_batch.)
-    int rc = ctx_ensure((void**)&ctx->d_ntt, &ctx->cap_ntt, bytes);
+    int rc = ctx->d_ntt.ensure(bytes);
     if (rc) return rc;
+    fe* d_ntt = ctx->d_ntt.at<fe>();
     // Only the first in_len coefficients of every polynomial cross PCIe (the kernels zero-pad by position), and for batches in
     // page-locked memory the three stages are pipelined over chunks of polynomials: copy-in of chunk k+1, the transform of
     // chunk k and the copy-out of chunk k-1 run on three streams.  16 x FFT(8n) of kimchi's quotient step (in_len = n) moves
@@ -761,10 +708,10 @@ int zk_ntt_batch(zk_ctx* root, int field_id, uint64_t* data, unsigned log_n, siz
         if (per * 2 > batch) per = (batch + 1) / 2;
     }
     if (per == batch) {
-        ZK_CUDA(cudaMemcpy2DAsync(ctx->d_ntt, poly_bytes, data, poly_bytes, in_len * sizeof(fe), batch, cudaMemcpyHostToDevice, ctx->stream));
-        rc = ctx_ntt_device(ctx, field_id, ctx->d_ntt, log_n, batch, in_len, inverse, coset);
+        ZK_CUDA(cudaMemcpy2DAsync(d_ntt, poly_bytes, data, poly_bytes, in_len * sizeof(fe), batch, cudaMemcpyHostToDevice, ctx->stream));
+        rc = ctx_ntt_device(ctx, field_id, d_ntt, log_n, batch, in_len, inverse, coset);
         if (rc) return rc;
-        ZK_CUDA(cudaMemcpyAsync(data, ctx->d_ntt, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        ZK_CUDA(cudaMemcpyAsync(data, d_ntt, bytes, cudaMemcpyDeviceToHost, ctx->stream));
         ZK_CUDA(cudaStreamSynchronize(ctx->stream));
         return ZK_OK;
     }
@@ -777,7 +724,7 @@ int zk_ntt_batch(zk_ctx* root, int field_id, uint64_t* data, unsigned log_n, siz
     if (e == cudaSuccess) e = cudaStreamWaitEvent(s_in, ctx->ev_fork, 0);
     for (size_t k = 0; k < chunks && e == cudaSuccess && rc == ZK_OK; k++) {
         const size_t j0 = k * per, cnt = std::min(per, batch - j0);
-        fe* d = ctx->d_ntt + j0 * n;
+        fe* d = d_ntt + j0 * n;
         const uint64_t* h = data + 4 * j0 * n;
         e = cudaEventCreateWithFlags(&ev[2 * k], cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev[2 * k + 1], cudaEventDisableTiming);
@@ -809,20 +756,17 @@ int zk_debug_field_op(zk_ctx* ctx, int field_id, int op, const uint64_t* a, cons
     if (!ctx || !a || !b || !out) { zk_set_error("null argument"); return ZK_ERR_INVALID; }
     std::lock_guard<std::mutex> lk(ctx->mu);
     ZK_CUDA(cudaSetDevice(ctx->device));
-    fe *da, *db, *dout;
-    ZK_CUDA(cudaMalloc(&da, n * sizeof(fe)));
-    ZK_CUDA(cudaMalloc(&db, n * sizeof(fe)));
-    ZK_CUDA(cudaMalloc(&dout, n * sizeof(fe)));
-    ZK_CUDA(cudaMemcpyAsync(da, a, n * sizeof(fe), cudaMemcpyHostToDevice, ctx->stream));
-    ZK_CUDA(cudaMemcpyAsync(db, b, n * sizeof(fe), cudaMemcpyHostToDevice, ctx->stream));
+    DevScratch da, db, dout;             // transient: freed on every return
+    int rc = da.ensure(n * sizeof(fe));
+    if (rc || (rc = db.ensure(n * sizeof(fe))) || (rc = dout.ensure(n * sizeof(fe)))) return rc;
+    ZK_CUDA(cudaMemcpyAsync(da.p, a, n * sizeof(fe), cudaMemcpyHostToDevice, ctx->stream));
+    ZK_CUDA(cudaMemcpyAsync(db.p, b, n * sizeof(fe), cudaMemcpyHostToDevice, ctx->stream));
     unsigned blocks = (unsigned)((n + 127) / 128);
-    if (field_id == ZK_FP) k_field_op<FpParams><<<blocks, 128, 0, ctx->stream>>>(op, da, db, dout, n);
-    else k_field_op<FqParams><<<blocks, 128, 0, ctx->stream>>>(op, da, db, dout, n);
+    with_field(field_id, [&](auto f) { k_field_op<typename decltype(f)::Dev><<<blocks, 128, 0, ctx->stream>>>(op, da.at<fe>(), db.at<fe>(), dout.at<fe>(), n); });
     ZK_CUDA(cudaGetLastError());
     ctx->launches += 1;
-    ZK_CUDA(cudaMemcpyAsync(out, dout, n * sizeof(fe), cudaMemcpyDeviceToHost, ctx->stream));
+    ZK_CUDA(cudaMemcpyAsync(out, dout.p, n * sizeof(fe), cudaMemcpyDeviceToHost, ctx->stream));
     ZK_CUDA(cudaStreamSynchronize(ctx->stream));
-    cudaFree(da); cudaFree(db); cudaFree(dout);
     return ZK_OK;
 }
 
@@ -835,32 +779,32 @@ int zk_debug_op_throughput(zk_ctx* ctx, int field_id, int kind, unsigned blocks,
     cudaDeviceProp prop;
     ZK_CUDA(cudaGetDeviceProperties(&prop, ctx->device));
     if (blocks == 0) blocks = prop.multiProcessorCount * 4;
-    xyzz_t* dout;
-    ZK_CUDA(cudaMalloc(&dout, sizeof(xyzz_t)));
-    cudaEvent_t e0, e1;
-    ZK_CUDA(cudaEventCreate(&e0));
-    ZK_CUDA(cudaEventCreate(&e1));
+    DevScratch dout;                     // transient, like the events: freed on every return
+    if (int rc = dout.ensure(sizeof(xyzz_t))) return rc;
+    xyzz_t* d = dout.at<xyzz_t>();
+    struct Event { cudaEvent_t e = nullptr; ~Event() { if (e) cudaEventDestroy(e); } } e0, e1;
+    ZK_CUDA(cudaEventCreate(&e0.e));
+    ZK_CUDA(cudaEventCreate(&e1.e));
     for (int rep = 0; rep < 2; rep++) {  // first launch warms up
-        ZK_CUDA(cudaEventRecord(e0, ctx->stream));
-#define LAUNCH(F)                                                                                        \
-        if (kind == 1) k_mul_chain<F, 1><<<blocks, threads, 0, ctx->stream>>>((fe*)dout, iters);         \
-        else if (kind == 2) k_mul_chain<F, 2><<<blocks, threads, 0, ctx->stream>>>((fe*)dout, iters);    \
-        else if (kind == 4) k_mul_chain<F, 4><<<blocks, threads, 0, ctx->stream>>>((fe*)dout, iters);    \
-        else if (kind == 101) k_add_chain<F, 1><<<blocks, threads, 0, ctx->stream>>>(dout, iters);                \
-        else if (kind == 102) k_add_chain<F, 0><<<blocks, threads, 0, ctx->stream>>>(dout, iters);                \
-        else k_madd_chain<F><<<blocks, threads, 0, ctx->stream>>>(dout, iters);
-        if (field_id == ZK_FP) { LAUNCH(FpParams) } else { LAUNCH(FqParams) }
-#undef LAUNCH
+        ZK_CUDA(cudaEventRecord(e0.e, ctx->stream));
+        with_field(field_id, [&](auto f) {
+            using F = typename decltype(f)::Dev;
+            if (kind == 1) k_mul_chain<F, 1><<<blocks, threads, 0, ctx->stream>>>((fe*)d, iters);
+            else if (kind == 2) k_mul_chain<F, 2><<<blocks, threads, 0, ctx->stream>>>((fe*)d, iters);
+            else if (kind == 4) k_mul_chain<F, 4><<<blocks, threads, 0, ctx->stream>>>((fe*)d, iters);
+            else if (kind == 101) k_add_chain<F, 1><<<blocks, threads, 0, ctx->stream>>>(d, iters);
+            else if (kind == 102) k_add_chain<F, 0><<<blocks, threads, 0, ctx->stream>>>(d, iters);
+            else k_madd_chain<F><<<blocks, threads, 0, ctx->stream>>>(d, iters);
+        });
         ZK_CUDA(cudaGetLastError());
-        ZK_CUDA(cudaEventRecord(e1, ctx->stream));
-        ZK_CUDA(cudaEventSynchronize(e1));
+        ZK_CUDA(cudaEventRecord(e1.e, ctx->stream));
+        ZK_CUDA(cudaEventSynchronize(e1.e));
     }
     ctx->launches += 2;
     float ms = 0;
-    ZK_CUDA(cudaEventElapsedTime(&ms, e0, e1));
+    ZK_CUDA(cudaEventElapsedTime(&ms, e0.e, e1.e));
     double per_thread = kind == 101 ? 0.25 : kind >= 100 ? 1.0 : (double)kind;
     *out_ops_per_s = per_thread * iters * (double)blocks * threads / (ms * 1e-3);
-    cudaEventDestroy(e0); cudaEventDestroy(e1); cudaFree(dout);
     return ZK_OK;
 }
 

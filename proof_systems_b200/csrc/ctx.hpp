@@ -1,12 +1,95 @@
-// ctx.hpp — the objects behind the opaque handles of include/zkb200.h.
+// ctx.hpp — the objects behind the opaque handles of include/zkb200.h, and the host-side helpers every entry point shares: the
+// field_id / curve_id dispatch, the argument checks and the context's scratch memory.
 #pragma once
 #include <map>
 #include <memory>
 #include <mutex>
 #include <vector>
 
+#include "host_field.hpp"
 #include "msm.cuh"
 #include "ntt.cuh"
+
+namespace zkb {
+// a field: its device parameters (field.cuh) and its host arithmetic (host_field.hpp)
+template <class D, class H, int ID> struct FieldTraits { using Dev = D; using Host = H; static constexpr int id = ID; };
+using FpTraits = FieldTraits<FpParams, host::HFp, ZK_FP>;
+using FqTraits = FieldTraits<FqParams, host::HFq, ZK_FQ>;
+
+// a curve: the fields of its coordinates (F device, HP host) and of its scalars (FS, HS)
+template <class B, class S> struct CurveTraits {
+    using Base = B; using Scalar = S;
+    using F = typename B::Dev; using HP = typename B::Host; using FS = typename S::Dev; using HS = typename S::Host;
+    static constexpr int scalar_field = S::id;
+};
+using PallasTraits = CurveTraits<FpTraits, FqTraits>;
+using VestaTraits = CurveTraits<FqTraits, FpTraits>;
+
+// fn(traits of the id): ZK_FP / ZK_PALLAS select the first type, any other id the second (check_field / check_curve refuse bad ids)
+template <class Fn> auto with_field(int field_id, Fn&& fn) { return field_id == ZK_FP ? fn(FpTraits{}) : fn(FqTraits{}); }
+template <class Fn> auto with_curve(int curve_id, Fn&& fn) { return curve_id == ZK_PALLAS ? fn(PallasTraits{}) : fn(VestaTraits{}); }
+
+inline int check_field(const char* what, int field_id) {
+    if (field_id != ZK_FP && field_id != ZK_FQ) { zk_set_error("%s: unknown field_id %d", what, field_id); return ZK_ERR_INVALID; }
+    return ZK_OK;
+}
+// what = null: the message has no prefix
+inline int check_curve(const char* what, int curve_id) {
+    if (curve_id == ZK_PALLAS || curve_id == ZK_VESTA) return ZK_OK;
+    what ? zk_set_error("%s: unknown curve_id %d", what, curve_id) : zk_set_error("unknown curve_id %d", curve_id);
+    return ZK_ERR_INVALID;
+}
+// domains of up to 2^30 points, the NTT's limit
+inline int check_log_n(const char* what, unsigned log_n, const char* name = "log_n") {
+    if (log_n > 30) { zk_set_error("%s: %s %u > 30", what, name, log_n); return ZK_ERR_INVALID; }
+    return ZK_OK;
+}
+// x (4 little-endian u64 limbs) is below the field's modulus
+inline bool canonical(int field_id, const uint64_t* x) {
+    return with_field(field_id, [&](auto f) { return !host::geq_mod<typename decltype(f)::Host>(x); });
+}
+
+// Memory that grows on demand (the contents are not kept) and is freed with its owner: device memory, or page-locked host memory
+// with PINNED.  zk_ctx_destroy makes the context's device current before its members are destroyed.
+template <bool PINNED> struct Scratch {
+    void* p = nullptr;
+    size_t cap = 0;
+    Scratch() = default;
+    Scratch(const Scratch&) = delete;
+    Scratch& operator=(const Scratch&) = delete;
+    ~Scratch() { release(); }
+    void release() {
+        if (p) PINNED ? cudaFreeHost(p) : cudaFree(p);
+        p = nullptr, cap = 0;
+    }
+    int ensure(size_t bytes) {
+        if (cap >= bytes) return ZK_OK;
+        release();
+        ZK_CUDA(PINNED ? cudaMallocHost(&p, bytes) : cudaMalloc(&p, bytes));
+        cap = bytes;
+        return ZK_OK;
+    }
+    template <class T> T* at(size_t byte_off = 0) const { return (T*)((char*)p + byte_off); }
+};
+using DevScratch = Scratch<false>;
+using PinnedScratch = Scratch<true>;
+
+// sub-buffers of one scratch allocation: add() hands out 256-byte aligned offsets in order, total is the size to ensure
+struct Layout {
+    size_t total = 0;
+    size_t add(size_t bytes) { const size_t off = (total + 255) & ~(size_t)255; total = off + bytes; return off; }
+};
+
+// a context's pinned slots for small read-backs (ctx_pinned), one per use
+struct PinnedSlots {
+    fe ip[2];                   // the IPA rounds' two inner products; zk_srs_open: the combined inner product, then a0
+    fe s0[2];                   // s_0 = (1) of the IPA rounds per curve, by scalar field id: the source of host-to-device copies that
+                                // nothing waits for, so it is only ever rewritten with the same value and never used for anything else
+    unsigned remainder;         // zk_poly_divide_by_vanishing_dev: nonzero remainder flag
+    unsigned long long ft_len;  // zk_prover_ft_dev: ft's length and ft(zeta omega)
+    fe ft_eval1;
+};
+}  // namespace zkb
 
 struct zk_ctx {
     // Concurrency (SURVEY.md §8b "Threading": SRS is Sync + Send, 15 rayon workers commit at once, kimchi/src/prover.rs:329-351):
@@ -29,36 +112,27 @@ struct zk_ctx {
     cudaStream_t side[SIDE_STREAMS] = {};
     int batch = (int)zkb::MSM_MAX_BATCH; // zk_ctx_set_option("msm_batch"): MSMs of one call fused into one pipeline
     cudaEvent_t ev_fork = nullptr;
-    zkb::fe* d_scalars = nullptr;        // staging for host-pointer MSM calls
-    size_t cap_scalars = 0;
-    zkb::fe* d_ntt = nullptr;            // staging for host-pointer NTT calls
-    size_t cap_ntt = 0;
-    zkb::fe* d_ntt_tmp = nullptr;        // second buffer of the two-pass plan
-    size_t cap_ntt_tmp = 0;
+    zkb::DevScratch d_scalars;           // staging for host-pointer MSM calls
+    zkb::DevScratch d_ntt;               // staging for host-pointer NTT calls
+    zkb::DevScratch d_ntt_tmp;           // second buffer of the two-pass plan
     zkb::fe* ntt_small[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};  // [field][inverse] w_1024^(+-i)
     std::map<unsigned, zkb::NttTables> ntt_tables;                         // key: field | inverse << 1 | log_n << 2
-    zkb::xyzz_t* d_gather_sum = nullptr; // zk_msm_finish_gathered: cross-rank sums of the slice sums
-    size_t cap_gather_sum = 0;
-    zkb::xyzz_t* h_gather = nullptr;     // ... and their pinned host copy
-    size_t cap_h_gather = 0;
-    void* h_scratch = nullptr;           // 256 pinned bytes for small read-backs
-    void* d_open = nullptr;              // zk_srs_open: staged polynomials | evaluation part | descriptors | extra bases
-    size_t cap_open = 0;
-    unsigned* d_flag = nullptr;          // zk_poly_divide_by_vanishing_dev: remainder flag
-    void* d_expr = nullptr;              // zk_expr_eval_dev: program | constants | column table
-    size_t cap_expr = 0;
-    void* d_ipa = nullptr;               // zk_srs_open: the rounds' state (a, b, challenge products, expanded scalars), kept between calls
-    size_t cap_ipa = 0;
-    void* d_verify = nullptr;            // zk_srs_verify: s vector | challenge tables | proof points and their scalars
-    size_t cap_verify = 0;
-    void* d_evals = nullptr;             // zk_lagrange_evaluate_dev / zk_poly_evaluate_chunks_dev: descriptors | partial sums | results
-    size_t cap_evals = 0;
-    void* d_ft = nullptr;                // zk_prover_ft_dev: f over d1 | term descriptors | length counter
-    size_t cap_ft = 0;
+    zkb::DevScratch d_gather_sum;        // zk_msm_finish_gathered: cross-rank sums of the slice sums
+    zkb::PinnedScratch h_gather;         // ... and their pinned host copy
+    zkb::PinnedScratch h_slots;          // zkb::PinnedSlots, through ctx_pinned
+    zkb::DevScratch d_open;              // zk_srs_open: staged polynomials | evaluation part | descriptors | extra bases
+    zkb::DevScratch d_flag;              // zk_poly_divide_by_vanishing_dev: remainder flag
+    zkb::DevScratch d_expr;              // zk_expr_eval_dev: program | constants | column table
+    zkb::DevScratch d_ipa;               // zk_srs_open: the rounds' state (a, b, challenge products, expanded scalars), kept between calls
+    zkb::DevScratch d_verify;            // zk_srs_verify: s vector | challenge tables | proof points and their scalars
+    zkb::DevScratch d_evals;             // zk_lagrange_evaluate_dev / zk_poly_evaluate_chunks_dev: descriptors | partial sums | results
+    zkb::DevScratch d_ft;                // zk_prover_ft_dev: f over d1 | term descriptors | length counter
     uint64_t launches = 0;
     bool profile = false;                // per-stage device timing (zk_ctx_set_profile)
     cudaEvent_t ev_ntt[2] = {nullptr, nullptr};
     float ntt_ms = 0;                    // device time of the last profiled NTT call (all its kernels)
+    // frees the scratch members; hidden like the library's other C++ symbols (zkb200.h gives the type default visibility)
+    __attribute__((visibility("hidden"))) ~zk_ctx() = default;
 };
 
 struct zk_bases {
@@ -77,7 +151,10 @@ inline zk_ctx* ctx_root(zk_ctx* c) { return c && c->parent ? c->parent : c; }
 inline const zk_ctx* ctx_root(const zk_ctx* c) { return c && c->parent ? c->parent : c; }
 int ctx_msm_device(zk_ctx* ctx, const zk_bases* bases, size_t off, size_t n, const fe* d_scalars, int mont, int window_bits,
                    uint64_t out_xyz[12]);
-int ctx_ensure(void** p, size_t* cap, size_t bytes);
+// the context's pinned slots, allocated on first use; null (the error set) when that fails
+inline PinnedSlots* ctx_pinned(zk_ctx* ctx) { return ctx->h_slots.ensure(sizeof(PinnedSlots)) ? nullptr : ctx->h_slots.at<PinnedSlots>(); }
+// the unscaled twiddle tables of a forward / inverse transform (pointwise evaluators take x_i = w^i from them)
+int ctx_ntt_table_ptrs(zk_ctx* ctx, int field, unsigned log_n, bool inverse, const fe** ulo, const fe** mid, const fe** hi2);
 // the NTT of zk_ntt_dev without the context lock (the caller holds it)
 int ctx_ntt_device(zk_ctx* ctx, int field, fe* d_data, unsigned log_n, size_t batch, size_t in_len, int inverse, int coset);
 int ctx_ntt_device_oop(zk_ctx* ctx, int field, const fe* d_in, size_t in_bs, fe* d_out, unsigned log_n, size_t batch, size_t in_len, int inverse, int coset);

@@ -237,14 +237,6 @@ template <class FS> int launch_sum(const fe* part, size_t nparts, fe* out, size_
     return ZK_OK;
 }
 
-int ctx_ntt_table_ptrs(zk_ctx* ctx, int field, unsigned log_n, bool inverse, const fe** ulo, const fe** mid, const fe** hi2);   // api.cu
-
-static bool canonical(int field, const uint64_t* x) {
-    fe v;
-    memcpy(&v, x, 32);
-    return field == ZK_FP ? fe_lt_modulus<FpParams>(v) : fe_lt_modulus<FqParams>(v);
-}
-
 template <class FS> static fe host_basis_scale(const fe& x, unsigned log_n) {
     // (x^n - 1) / n: the numerator of batch_inversion_and_mul over t_0 = prod_{j>=1} (1 - w^j) = n
     fe n = fe_zero();
@@ -270,25 +262,27 @@ int ctx_evaluate_chunks(zk_ctx* ctx, int field_id, const zk_dev_poly* polys, siz
     if (n_cov == 0) return ZK_OK;
     cudaStream_t st = ctx->stream;
     // context scratch: polynomial table | points | partial sums | results
-    const size_t b_pol = ((n_polys * sizeof(DevPoly)) + 255) & ~(size_t)255, b_pts = ((n_points * sizeof(fe)) + 255) & ~(size_t)255;
-    const size_t o_part = b_pol + b_pts, o_res = o_part + n_cov * bpc * sizeof(fe), total = o_res + n_cov * sizeof(fe);
-    int rc = ctx_ensure(&ctx->d_evals, &ctx->cap_evals, total);
+    Layout lay;
+    const size_t o_pol = lay.add(n_polys * sizeof(DevPoly)), o_pts = lay.add(n_points * sizeof(fe));
+    const size_t o_part = lay.add(n_cov * bpc * sizeof(fe)), o_res = lay.add(n_cov * sizeof(fe));
+    int rc = ctx->d_evals.ensure(lay.total);
     if (rc) return rc;
-    stage.assign(b_pol + b_pts, 0);
+    stage.assign(o_part, 0);
     for (size_t k = 0; k < n_polys; k++) {
         const DevPoly d{(const fe*)polys[k].d_coeffs, polys[k].len};
-        memcpy(stage.data() + k * sizeof(DevPoly), &d, sizeof(DevPoly));
+        memcpy(stage.data() + o_pol + k * sizeof(DevPoly), &d, sizeof(DevPoly));
     }
-    memcpy(stage.data() + b_pol, points_mont, n_points * sizeof(fe));
-    uint8_t* base = (uint8_t*)ctx->d_evals;
-    ZK_CUDA(cudaMemcpyAsync(base, stage.data(), stage.size(), cudaMemcpyHostToDevice, st));
+    memcpy(stage.data() + o_pts, points_mont, n_points * sizeof(fe));
+    ZK_CUDA(cudaMemcpyAsync(ctx->d_evals.p, stage.data(), stage.size(), cudaMemcpyHostToDevice, st));
     ChunkEvalArgs a{};
-    a.polys = (const DevPoly*)base; a.points = (const fe*)(base + b_pol); a.partial = (fe*)(base + o_part);
+    a.polys = ctx->d_evals.at<const DevPoly>(o_pol); a.points = ctx->d_evals.at<const fe>(o_pts); a.partial = ctx->d_evals.at<fe>(o_part);
     a.chunk_size = chunk_size; a.n_points = (unsigned)n_points; a.covered = (unsigned)covered; a.spc = (unsigned)spc; a.bpc = (unsigned)bpc;
     const dim3 grid((unsigned)(covered * bpc), (unsigned)n_polys, (unsigned)((n_points + HS_PTS - 1) / HS_PTS));
-    fe* res = (fe*)(base + o_res);
-    if (field_id == ZK_FP) { k_evaluate_chunks<FpParams><<<grid, EV_THREADS, 0, st>>>(a); rc = launch_sum<FpParams>(a.partial, bpc, res, n_cov, st); }
-    else { k_evaluate_chunks<FqParams><<<grid, EV_THREADS, 0, st>>>(a); rc = launch_sum<FqParams>(a.partial, bpc, res, n_cov, st); }
+    fe* res = ctx->d_evals.at<fe>(o_res);
+    rc = with_field(field_id, [&](auto f) {
+        using FS = typename decltype(f)::Dev;
+        k_evaluate_chunks<FS><<<grid, EV_THREADS, 0, st>>>(a); return launch_sum<FS>(a.partial, bpc, res, n_cov, st);
+    });
     if (rc) return rc;
     ctx->launches += 1 + (n_cov + 65534) / 65535;
     *d_res = res;
@@ -307,8 +301,8 @@ size_t zk_lagrange_evals_chunks(size_t domain_size, size_t max_poly_size) {
 
 int zk_lagrange_evals_dev(zk_ctx* ctx, int field_id, unsigned log_n, size_t max_poly_size, const uint64_t x_mont[4], void* d_out) {
     if (!ctx || !x_mont || !d_out) { zk_set_error("lagrange_evals: null argument"); return ZK_ERR_INVALID; }
-    if (field_id != ZK_FP && field_id != ZK_FQ) { zk_set_error("lagrange_evals: unknown field_id %d", field_id); return ZK_ERR_INVALID; }
-    if (log_n > 30) { zk_set_error("lagrange_evals: log_n %u > 30", log_n); return ZK_ERR_INVALID; }
+    if (int rc = check_field("lagrange_evals", field_id)) return rc;
+    if (int rc = check_log_n("lagrange_evals", log_n)) return rc;
     if (max_poly_size == 0) { zk_set_error("lagrange_evals: max_poly_size is 0"); return ZK_ERR_INVALID; }
     const size_t n = (size_t)1 << log_n, chunks = zk_lagrange_evals_chunks(n, max_poly_size);
     if (chunks == 0) { zk_set_error("lagrange_evals: domain size %zu is not a multiple of max_poly_size %zu", n, max_poly_size); return ZK_ERR_INVALID; }
@@ -324,18 +318,18 @@ int zk_lagrange_evals_dev(zk_ctx* ctx, int field_id, unsigned log_n, size_t max_
         if (rc) return rc;
         a.out = (fe*)d_out; a.n = n; a.x = x;
         a.threads = (n + LB_SEG - 1) / LB_SEG;
-        a.c = field_id == ZK_FP ? host_basis_scale<FpParams>(x, log_n) : host_basis_scale<FqParams>(x, log_n);
         const unsigned blocks = (unsigned)((a.threads + EV_THREADS - 1) / EV_THREADS);
-        if (field_id == ZK_FP) k_lagrange_basis<FpParams><<<blocks, EV_THREADS, 0, st>>>(a);
-        else k_lagrange_basis<FqParams><<<blocks, EV_THREADS, 0, st>>>(a);
+        with_field(field_id, [&](auto f) {
+            using FS = typename decltype(f)::Dev;
+            a.c = host_basis_scale<FS>(x, log_n); k_lagrange_basis<FS><<<blocks, EV_THREADS, 0, st>>>(a);
+        });
         ZK_CUDA(cudaGetLastError());
         ctx->launches += 1;
         return ZK_OK;
     }
     const size_t total = chunks * n, threads = (total + LB_RUN - 1) / LB_RUN;
     const unsigned blocks = (unsigned)((threads + EV_THREADS - 1) / EV_THREADS);
-    if (field_id == ZK_FP) k_chunked_powers<FpParams><<<blocks, EV_THREADS, 0, st>>>((fe*)d_out, log_n, max_poly_size, total, x);
-    else k_chunked_powers<FqParams><<<blocks, EV_THREADS, 0, st>>>((fe*)d_out, log_n, max_poly_size, total, x);
+    with_field(field_id, [&](auto f) { k_chunked_powers<typename decltype(f)::Dev><<<blocks, EV_THREADS, 0, st>>>((fe*)d_out, log_n, max_poly_size, total, x); });
     ZK_CUDA(cudaGetLastError());
     ctx->launches += 1;
     return ctx_ntt_device(ctx, field_id, (fe*)d_out, log_n, chunks, 0, /* inverse = */ 1, /* coset = */ 0);
@@ -344,8 +338,8 @@ int zk_lagrange_evals_dev(zk_ctx* ctx, int field_id, unsigned log_n, size_t max_
 int zk_lagrange_evaluate_dev(zk_ctx* ctx, int field_id, const void* const* d_bases, size_t n_points, unsigned log_n, size_t chunks,
                              const zk_eval_column* cols, size_t n_cols, uint64_t* out) {
     if (!ctx || (!d_bases && n_points) || (!cols && n_cols) || (!out && n_points && n_cols)) { zk_set_error("lagrange_evaluate: null argument"); return ZK_ERR_INVALID; }
-    if (field_id != ZK_FP && field_id != ZK_FQ) { zk_set_error("lagrange_evaluate: unknown field_id %d", field_id); return ZK_ERR_INVALID; }
-    if (log_n > 30) { zk_set_error("lagrange_evaluate: log_n %u > 30", log_n); return ZK_ERR_INVALID; }
+    if (int rc = check_field("lagrange_evaluate", field_id)) return rc;
+    if (int rc = check_log_n("lagrange_evaluate", log_n)) return rc;
     const size_t n = (size_t)1 << log_n;
     // a basis of D(n) has 1 vector, or n / max_poly_size for a divisor max_poly_size < n: chunks divides n either way
     if (chunks == 0 || chunks > n || n % chunks) { zk_set_error("lagrange_evaluate: %zu chunks cannot belong to a basis of a domain of %zu", chunks, n); return ZK_ERR_INVALID; }
@@ -374,22 +368,24 @@ int zk_lagrange_evaluate_dev(zk_ctx* ctx, int field_id, const void* const* d_bas
     const unsigned blocks_x = (unsigned)std::min<size_t>(std::min(by_len, by_fill), 65535);
     const size_t n_out = n_cols * n_pairs;
     // context scratch: column table | basis pointers | partial sums | results
-    const size_t b_col = ((n_cols * sizeof(EvalCol)) + 255) & ~(size_t)255, b_bas = ((n_points * sizeof(fe*)) + 255) & ~(size_t)255;
-    const size_t o_part = b_col + b_bas, o_res = o_part + n_out * blocks_x * sizeof(fe), total = o_res + n_out * sizeof(fe);
-    int rc = ctx_ensure(&ctx->d_evals, &ctx->cap_evals, total);
+    Layout lay;
+    const size_t o_col = lay.add(n_cols * sizeof(EvalCol)), o_bas = lay.add(n_points * sizeof(fe*));
+    const size_t o_part = lay.add(n_out * blocks_x * sizeof(fe)), o_res = lay.add(n_out * sizeof(fe));
+    int rc = ctx->d_evals.ensure(lay.total);
     if (rc) return rc;
-    std::vector<uint8_t> stage(b_col + b_bas, 0);
-    memcpy(stage.data(), hc.data(), n_cols * sizeof(EvalCol));
-    memcpy(stage.data() + b_col, d_bases, n_points * sizeof(fe*));
-    uint8_t* base = (uint8_t*)ctx->d_evals;
-    ZK_CUDA(cudaMemcpyAsync(base, stage.data(), stage.size(), cudaMemcpyHostToDevice, st));
+    std::vector<uint8_t> stage(o_part, 0);
+    memcpy(stage.data() + o_col, hc.data(), n_cols * sizeof(EvalCol));
+    memcpy(stage.data() + o_bas, d_bases, n_points * sizeof(fe*));
+    ZK_CUDA(cudaMemcpyAsync(ctx->d_evals.p, stage.data(), stage.size(), cudaMemcpyHostToDevice, st));
     LagEvalArgs a{};
-    a.cols = (const EvalCol*)base; a.bases = (const fe* const*)(base + b_col); a.partial = (fe*)(base + o_part);
+    a.cols = ctx->d_evals.at<const EvalCol>(o_col); a.bases = ctx->d_evals.at<const fe* const>(o_bas); a.partial = ctx->d_evals.at<fe>(o_part);
     a.n = n; a.chunks = (unsigned)chunks; a.n_pairs = (unsigned)n_pairs; a.blocks_x = blocks_x;
     const dim3 grid(blocks_x, (unsigned)n_cols, (unsigned)groups);
-    fe* res = (fe*)(base + o_res);
-    if (field_id == ZK_FP) { k_lagrange_evaluate<FpParams><<<grid, EV_THREADS, 0, st>>>(a); rc = launch_sum<FpParams>(a.partial, blocks_x, res, n_out, st); }
-    else { k_lagrange_evaluate<FqParams><<<grid, EV_THREADS, 0, st>>>(a); rc = launch_sum<FqParams>(a.partial, blocks_x, res, n_out, st); }
+    fe* res = ctx->d_evals.at<fe>(o_res);
+    rc = with_field(field_id, [&](auto f) {
+        using FS = typename decltype(f)::Dev;
+        k_lagrange_evaluate<FS><<<grid, EV_THREADS, 0, st>>>(a); return launch_sum<FS>(a.partial, blocks_x, res, n_out, st);
+    });
     if (rc) return rc;
     ctx->launches += 1 + (n_out + 65534) / 65535;
     ZK_CUDA(cudaMemcpyAsync(out, res, n_out * sizeof(fe), cudaMemcpyDeviceToHost, st));
@@ -400,7 +396,7 @@ int zk_lagrange_evaluate_dev(zk_ctx* ctx, int field_id, const void* const* d_bas
 int zk_poly_evaluate_chunks_dev(zk_ctx* ctx, int field_id, const zk_dev_poly* polys, size_t n_polys, size_t num_chunks, size_t chunk_size,
                                 const uint64_t* points_mont, size_t n_points, uint64_t* out) {
     if (!ctx || (!polys && n_polys) || (!points_mont && n_points) || (!out && n_polys && n_points && num_chunks)) { zk_set_error("evaluate_chunks: null argument"); return ZK_ERR_INVALID; }
-    if (field_id != ZK_FP && field_id != ZK_FQ) { zk_set_error("evaluate_chunks: unknown field_id %d", field_id); return ZK_ERR_INVALID; }
+    if (int rc = check_field("evaluate_chunks", field_id)) return rc;
     if (chunk_size == 0) { zk_set_error("evaluate_chunks: chunk_size is 0"); return ZK_ERR_INVALID; }
     if (n_polys > 65535) { zk_set_error("evaluate_chunks: %zu polynomials, at most 65535", n_polys); return ZK_ERR_INVALID; }
     if (n_points > (size_t)65535 * HS_PTS) { zk_set_error("evaluate_chunks: %zu points, at most %u", n_points, 65535 * HS_PTS); return ZK_ERR_INVALID; }

@@ -105,7 +105,7 @@ extern "C" int zk_expr_eval_dev(zk_ctx* ctx, int field_id, const zk_expr_token* 
                                 size_t n_constants, const zk_expr_column* cols, size_t n_cols, uint64_t out_len, unsigned out_domain_mult,
                                 int accumulate, void* d_out) {
     if (!ctx || !tokens || (!constants_mont && n_constants) || (!cols && n_cols) || !d_out) { zk_set_error("expr_eval: null argument"); return ZK_ERR_INVALID; }
-    if (field_id != ZK_FP && field_id != ZK_FQ) { zk_set_error("expr_eval: unknown field_id %d", field_id); return ZK_ERR_INVALID; }
+    if (int rc = check_field("expr_eval", field_id)) return rc;
     if (out_len == 0 || (out_len & (out_len - 1)) || out_len > ((uint64_t)1 << 30)) { zk_set_error("expr_eval: output domain size %llu is not a power of two <= 2^30", (unsigned long long)out_len); return ZK_ERR_INVALID; }
     if (out_domain_mult == 0 || (out_domain_mult & (out_domain_mult - 1)) || out_len % out_domain_mult) { zk_set_error("expr_eval: output domain multiple %u does not divide %llu", out_domain_mult, (unsigned long long)out_len); return ZK_ERR_INVALID; }
     if (n_tokens == 0 || n_tokens > (1u << 20)) { zk_set_error("expr_eval: %zu tokens outside [1, 2^20]", n_tokens); return ZK_ERR_INVALID; }
@@ -146,28 +146,27 @@ extern "C" int zk_expr_eval_dev(zk_ctx* ctx, int field_id, const zk_expr_token* 
     ZK_CUDA(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     // program, constants and column table in one staging buffer
-    const size_t b_tok = n_tokens * sizeof(zk_expr_token), b_con = std::max<size_t>(n_constants, 1) * sizeof(fe), b_col = std::max<size_t>(n_cols, 1) * sizeof(ExprCol);
-    const size_t o_con = (b_tok + 31) & ~(size_t)31, o_col = o_con + b_con, total = o_col + b_col;
-    int rc = ctx_ensure(&ctx->d_expr, &ctx->cap_expr, total);
-    if (rc) return rc;
-    std::vector<uint8_t> stage(total, 0);
-    memcpy(stage.data(), tokens, b_tok);
+    Layout lay;
+    const size_t o_tok = lay.add(n_tokens * sizeof(zk_expr_token)), o_con = lay.add(std::max<size_t>(n_constants, 1) * sizeof(fe));
+    const size_t o_col = lay.add(std::max<size_t>(n_cols, 1) * sizeof(ExprCol));
+    if (int rc = ctx->d_expr.ensure(lay.total)) return rc;
+    std::vector<uint8_t> stage(lay.total, 0);
+    memcpy(stage.data() + o_tok, tokens, n_tokens * sizeof(zk_expr_token));
     if (n_constants) memcpy(stage.data() + o_con, constants_mont, n_constants * sizeof(fe));
     if (n_cols) memcpy(stage.data() + o_col, hc.data(), n_cols * sizeof(ExprCol));
-    ZK_CUDA(cudaMemcpyAsync(ctx->d_expr, stage.data(), total, cudaMemcpyHostToDevice, st));
+    ZK_CUDA(cudaMemcpyAsync(ctx->d_expr.p, stage.data(), stage.size(), cudaMemcpyHostToDevice, st));
     ZK_CUDA(cudaStreamSynchronize(st));      // `stage` is a local
     ExprArgs a{};
-    a.tokens = (const zk_expr_token*)ctx->d_expr;
-    a.constants = (const fe*)((const uint8_t*)ctx->d_expr + o_con);
-    a.cols = (const ExprCol*)((const uint8_t*)ctx->d_expr + o_col);
+    a.tokens = ctx->d_expr.at<const zk_expr_token>(o_tok);
+    a.constants = ctx->d_expr.at<const fe>(o_con);
+    a.cols = ctx->d_expr.at<const ExprCol>(o_col);
     a.out = (fe*)d_out; a.out_len = out_len; a.n_tokens = (uint32_t)n_tokens; a.accumulate = accumulate ? 1 : 0;
     // one resident wave of threads striding over the domain: the local-memory frames (stack + cache) are reserved per resident thread
     int sms = 0;
     ZK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device));
     const uint64_t want = (out_len + 127) / 128;
     const unsigned blocks = (unsigned)std::min<uint64_t>(want, (uint64_t)sms * 8);
-    if (field_id == ZK_FP) k_expr_eval<FpParams><<<blocks, 128, 0, st>>>(a);
-    else k_expr_eval<FqParams><<<blocks, 128, 0, st>>>(a);
+    with_field(field_id, [&](auto f) { k_expr_eval<typename decltype(f)::Dev><<<blocks, 128, 0, st>>>(a); });
     ZK_CUDA(cudaGetLastError());
     ctx->launches += 1;
     return ZK_OK;

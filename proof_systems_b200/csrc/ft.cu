@@ -16,7 +16,6 @@
 #include <vector>
 
 #include "../../include/zkb200.h"
-#include "host_field.hpp"
 #include "poly.cuh"
 
 using namespace zkb;
@@ -34,12 +33,11 @@ __global__ void __launch_bounds__(FT_THREADS) k_last_nonzero(const fe* __restric
     if ((threadIdx.x & 31) == 0 && v) atomicMax(out, v);
 }
 
-template <class HP> static bool canonical(const uint64_t* x) { return !host::geq_mod<HP>(x); }
-
-template <class FS, class HP>
-static int ft_impl(zk_ctx* ctx, int field_id, unsigned log_n, size_t m, std::vector<CombineDesc>& terms, const fe* d_t, size_t t_len,
-                   const uint64_t zeta_mont[4], fe* d_ft, size_t* ft_len, uint64_t ft_eval1[4]) {
+template <class T>
+static int ft_impl(zk_ctx* ctx, unsigned log_n, size_t m, std::vector<CombineDesc>& terms, const fe* d_t, size_t t_len, const uint64_t zeta_mont[4],
+                   fe* d_ft, size_t* ft_len, uint64_t ft_eval1[4]) {
     using namespace host;
+    using FS = typename T::Dev; using HP = typename T::Host;
     const size_t n = (size_t)1 << log_n;
     // host scalars: zeta^m, -(zeta^n - 1) = 1 - zeta^n, zeta omega (omega: the generator of d1)
     hfe zeta;
@@ -52,23 +50,26 @@ static int ft_impl(zk_ctx* ctx, int field_id, unsigned log_n, size_t m, std::vec
     std::lock_guard<std::mutex> lk(ctx->mu);
     ZK_CUDA(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
-    if (!ctx->h_scratch) ZK_CUDA(cudaMallocHost(&ctx->h_scratch, 256));
+    PinnedSlots* pin = ctx_pinned(ctx);
+    if (!pin) return ZK_ERR_CUDA;
     // context scratch: f (n elements, only with terms) | term descriptors | the length counter
-    const size_t f_elems = terms.empty() ? 0 : n, o_desc = f_elems * sizeof(fe), o_len = o_desc + terms.size() * sizeof(CombineDesc);
-    int rc = ctx_ensure(&ctx->d_ft, &ctx->cap_ft, o_len + sizeof(unsigned long long));
+    Layout lay;
+    const size_t o_f = lay.add((terms.empty() ? 0 : n) * sizeof(fe)), o_desc = lay.add(terms.size() * sizeof(CombineDesc));
+    const size_t o_len = lay.add(sizeof(unsigned long long));
+    int rc = ctx->d_ft.ensure(lay.total);
     if (rc) return rc;
-    uint8_t* base = (uint8_t*)ctx->d_ft;
-    fe* d_f = (fe*)base;
-    unsigned long long* d_len = (unsigned long long*)(base + o_len);
+    fe* d_f = ctx->d_ft.at<fe>(o_f);
+    CombineDesc* d_desc = ctx->d_ft.at<CombineDesc>(o_desc);
+    unsigned long long* d_len = ctx->d_ft.at<unsigned long long>(o_len);
     ZK_CUDA(cudaMemsetAsync(d_len, 0, sizeof(unsigned long long), st));
     ZK_CUDA(cudaMemsetAsync(d_ft, 0, m * sizeof(fe), st));
     const unsigned lin_blocks = (unsigned)((m + FT_THREADS - 1) / FT_THREADS);
     if (!terms.empty()) {                         // f = 0 without terms: it adds nothing
-        ZK_CUDA(cudaMemcpyAsync(base + o_desc, terms.data(), terms.size() * sizeof(CombineDesc), cudaMemcpyHostToDevice, st));
-        k_combine<FS><<<(unsigned)((n + FT_THREADS - 1) / FT_THREADS), FT_THREADS, 0, st>>>((const CombineDesc*)(base + o_desc), (unsigned)terms.size(), d_f, n);
+        ZK_CUDA(cudaMemcpyAsync(d_desc, terms.data(), terms.size() * sizeof(CombineDesc), cudaMemcpyHostToDevice, st));
+        k_combine<FS><<<(unsigned)((n + FT_THREADS - 1) / FT_THREADS), FT_THREADS, 0, st>>>(d_desc, (unsigned)terms.size(), d_f, n);
         ZK_CUDA(cudaGetLastError());
         ctx->launches += 1;
-        rc = ctx_ntt_device(ctx, field_id, d_f, log_n, 1, 0, /* inverse = */ 1, /* coset = */ 0);     // Evaluations::interpolate
+        rc = ctx_ntt_device(ctx, T::id, d_f, log_n, 1, 0, /* inverse = */ 1, /* coset = */ 0);     // Evaluations::interpolate
         if (rc) return rc;
         k_linearize_add<FS><<<lin_blocks, FT_THREADS, 0, st>>>(d_ft, d_f, n, m, (unsigned)((n + m - 1) / m), fzm, fone);
         ZK_CUDA(cudaGetLastError());
@@ -86,16 +87,13 @@ static int ft_impl(zk_ctx* ctx, int field_id, unsigned log_n, size_t m, std::vec
     std::vector<uint8_t> stage;
     const fe* d_eval = nullptr;
     uint64_t covered = 0;
-    rc = ctx_evaluate_chunks(ctx, field_id, &ft, 1, m, zeta_omega.l, 1, stage, &d_eval, &covered);
+    rc = ctx_evaluate_chunks(ctx, T::id, &ft, 1, m, zeta_omega.l, 1, stage, &d_eval, &covered);
     if (rc) return rc;
-    uint8_t* h = (uint8_t*)ctx->h_scratch;        // bytes 208..255: the length, then ft(zeta omega)
-    ZK_CUDA(cudaMemcpyAsync(h + 208, d_len, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-    ZK_CUDA(cudaMemcpyAsync(h + 224, d_eval, sizeof(fe), cudaMemcpyDeviceToHost, st));
+    ZK_CUDA(cudaMemcpyAsync(&pin->ft_len, d_len, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    ZK_CUDA(cudaMemcpyAsync(&pin->ft_eval1, d_eval, sizeof(fe), cudaMemcpyDeviceToHost, st));
     ZK_CUDA(cudaStreamSynchronize(st));
-    unsigned long long len;
-    memcpy(&len, h + 208, sizeof(len));
-    *ft_len = (size_t)len;
-    memcpy(ft_eval1, h + 224, 32);
+    *ft_len = (size_t)pin->ft_len;
+    memcpy(ft_eval1, &pin->ft_eval1, 32);
     return ZK_OK;
 }
 
@@ -104,13 +102,12 @@ static int ft_impl(zk_ctx* ctx, int field_id, unsigned log_n, size_t m, std::vec
 extern "C" int zk_prover_ft_dev(zk_ctx* ctx, int field_id, unsigned log_n, size_t max_poly_size, const zk_lin_term* terms, size_t n_terms,
                                 const void* d_t, size_t t_len, const uint64_t zeta_mont[4], void* d_ft, size_t* ft_len, uint64_t ft_eval1[4]) {
     if (!ctx || (!terms && n_terms) || (!d_t && t_len) || !zeta_mont || !d_ft || !ft_len || !ft_eval1) { zk_set_error("prover_ft: null argument"); return ZK_ERR_INVALID; }
-    if (field_id != ZK_FP && field_id != ZK_FQ) { zk_set_error("prover_ft: unknown field_id %d", field_id); return ZK_ERR_INVALID; }
-    if (log_n > 30) { zk_set_error("prover_ft: log_n %u > 30", log_n); return ZK_ERR_INVALID; }
+    if (int rc = check_field("prover_ft", field_id)) return rc;
+    if (int rc = check_log_n("prover_ft", log_n)) return rc;
     if (max_poly_size == 0) { zk_set_error("prover_ft: max_poly_size is 0"); return ZK_ERR_INVALID; }
     const size_t n = (size_t)1 << log_n, m = max_poly_size;
     if (n >= m && n % m) { zk_set_error("prover_ft: domain size %zu is not a multiple of max_poly_size %zu", n, m); return ZK_ERR_INVALID; }
-    const bool fp = field_id == ZK_FP;
-    if (!(fp ? canonical<host::HFp>(zeta_mont) : canonical<host::HFq>(zeta_mont))) { zk_set_error("prover_ft: zeta is not a canonical field element"); return ZK_ERR_INVALID; }
+    if (!canonical(field_id, zeta_mont)) { zk_set_error("prover_ft: zeta is not a canonical field element"); return ZK_ERR_INVALID; }
     if (n_terms > 0xffffffffu) { zk_set_error("prover_ft: %zu terms are too many", n_terms); return ZK_ERR_INVALID; }
     std::vector<CombineDesc> descs(n_terms);
     for (size_t k = 0; k < n_terms; k++) {
@@ -118,7 +115,7 @@ extern "C" int zk_prover_ft_dev(zk_ctx* ctx, int field_id, unsigned log_n, size_
         if (!t.d_evals) { zk_set_error("prover_ft: term %zu is null", k); return ZK_ERR_INVALID; }
         // CombineDesc's 32-bit stride: kimchi's domains d1 .. d8 (len = n, 2n, 4n or 8n; 3n ... 7n are accepted too)
         if (t.len == 0 || t.len % n || t.len / n > 8) { zk_set_error("prover_ft: term %zu has %llu evaluations, not 1 .. 8 times %zu", k, (unsigned long long)t.len, n); return ZK_ERR_INVALID; }
-        if (!(fp ? canonical<host::HFp>(t.coeff) : canonical<host::HFq>(t.coeff))) { zk_set_error("prover_ft: coefficient of term %zu is not a canonical field element", k); return ZK_ERR_INVALID; }
+        if (!canonical(field_id, t.coeff)) { zk_set_error("prover_ft: coefficient of term %zu is not a canonical field element", k); return ZK_ERR_INVALID; }
         descs[k].p = (const fe*)t.d_evals;
         descs[k].len = (uint32_t)n;
         descs[k].stride = (uint32_t)(t.len / n);
@@ -129,6 +126,5 @@ extern "C" int zk_prover_ft_dev(zk_ctx* ctx, int field_id, unsigned log_n, size_
         zk_set_error("prover_ft: t has %zu coefficients, more than %zu chunks of %zu", t_len, 7 * num_chunks, m);
         return ZK_ERR_LENGTH;
     }
-    if (fp) return ft_impl<FpParams, host::HFp>(ctx, field_id, log_n, m, descs, (const fe*)d_t, t_len, zeta_mont, (fe*)d_ft, ft_len, ft_eval1);
-    return ft_impl<FqParams, host::HFq>(ctx, field_id, log_n, m, descs, (const fe*)d_t, t_len, zeta_mont, (fe*)d_ft, ft_len, ft_eval1);
+    return with_field(field_id, [&](auto f) { return ft_impl<decltype(f)>(ctx, log_n, m, descs, (const fe*)d_t, t_len, zeta_mont, (fe*)d_ft, ft_len, ft_eval1); });
 }

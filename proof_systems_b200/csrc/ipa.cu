@@ -18,7 +18,6 @@
 #include <mutex>
 
 #include "../../include/zkb200.h"
-#include "host_field.hpp"
 #include "ipa.hpp"
 #include "msm.cuh"
 
@@ -130,22 +129,19 @@ size_t ipa_storage_bytes(size_t n) { return (6 * n + 4 + IP_BLOCKS + 2) * sizeof
 int ipa_create(zk_ctx* ctx, const zk_bases* bases, size_t n, zk_ipa** out, void* storage) {
     if (n < 1 || (n & (n - 1))) { zk_set_error("ipa: n must be a power of two (the reference pads to a power of two, ipa.rs:848-850)"); return ZK_ERR_INVALID; }
     if (bases->b.n > n || (n > 1 && 2 * bases->b.n <= n)) { zk_set_error("ipa: n = %zu is not the SRS size %zu rounded up to a power of two", n, bases->b.n); return ZK_ERR_INVALID; }
+    PinnedSlots* pin = ctx_pinned(ctx);
+    if (!pin) return ZK_ERR_CUDA;
     zk_ipa* s = new zk_ipa();
     s->ctx = ctx; s->curve = bases->b.curve; s->n = s->n0 = n; s->bases = bases;
-    const fe one = s->curve == ZK_PALLAS ? fe_one<FqParams>() : fe_one<FpParams>();
     cudaError_t e = cudaSuccess;
     if (storage) { s->d_a = (fe*)storage; s->owns_storage = false; }
     else e = cudaMalloc(&s->d_a, ipa_storage_bytes(n));
     if (e == cudaSuccess) {
         s->d_b = s->d_a + n; s->d_s[0] = s->d_a + 2 * n; s->d_s[1] = s->d_a + 3 * n; s->d_sc = s->d_a + 4 * n; s->d_part = s->d_a + 6 * n + 4;
-        if (!ctx->h_scratch) e = cudaMallocHost(&ctx->h_scratch, 256);
-        s->h_ip = (fe*)ctx->h_scratch;
-    }
-    if (e == cudaSuccess) {
-        // s_0 = (1): staged through the context's pinned scratch (one slot per curve: the value never changes), nothing waits for the copy
-        char* slot = (char*)ctx->h_scratch + (s->curve == ZK_PALLAS ? 128 : 160);
-        memcpy(slot, &one, sizeof(fe));
-        e = cudaMemcpyAsync(s->d_s[0], slot, sizeof(fe), cudaMemcpyHostToDevice, ctx->stream);
+        s->h_ip = pin->ip;
+        // s_0 = (1), staged through the curve's slot (PinnedSlots::s0)
+        const fe* one = with_curve(s->curve, [&](auto c) { using C = decltype(c); return &(pin->s0[C::scalar_field] = fe_one<typename C::FS>()); });
+        e = cudaMemcpyAsync(s->d_s[0], one, sizeof(fe), cudaMemcpyHostToDevice, ctx->stream);
     }
     if (e != cudaSuccess) {
         zk_set_error("ipa: %s", cudaGetErrorString(e));
@@ -160,16 +156,14 @@ int ipa_round_lr(zk_ipa* s, uint64_t out_l_xyz[12], uint64_t out_r_xyz[12], uint
     if (s->n < 2) { zk_set_error("ipa_round_lr: folding is complete"); return ZK_ERR_INVALID; }
     zk_ctx* ctx = s->ctx;
     const size_t h = s->n / 2;
-    const bool pallas = s->curve == ZK_PALLAS;   // scalar field of Pallas is Fq
-    // inner products <a_hi, b_lo>, <a_lo, b_hi>
-    int rc = pallas ? ipa_inner_product<FqParams>(s, s->d_a + h, s->d_b, h, s->d_part + IP_BLOCKS)
-                    : ipa_inner_product<FpParams>(s, s->d_a + h, s->d_b, h, s->d_part + IP_BLOCKS);
-    if (rc) return rc;
-    rc = pallas ? ipa_inner_product<FqParams>(s, s->d_a, s->d_b + h, h, s->d_part + IP_BLOCKS + 1)
-                : ipa_inner_product<FpParams>(s, s->d_a, s->d_b + h, h, s->d_part + IP_BLOCKS + 1);
-    if (rc) return rc;
-    if (out_ip_l) ZK_CUDA(cudaMemcpyAsync(s->h_ip, s->d_part + IP_BLOCKS, 2 * sizeof(fe), cudaMemcpyDeviceToHost, ctx->stream));
-    rc = pallas ? ipa_expand_and_msm<FqParams>(s, h, out_l_xyz, out_r_xyz) : ipa_expand_and_msm<FpParams>(s, h, out_l_xyz, out_r_xyz);
+    int rc = with_curve(s->curve, [&](auto c) {
+        using FS = typename decltype(c)::FS;
+        // inner products <a_hi, b_lo>, <a_lo, b_hi>
+        if (int e = ipa_inner_product<FS>(s, s->d_a + h, s->d_b, h, s->d_part + IP_BLOCKS)) return e;
+        if (int e = ipa_inner_product<FS>(s, s->d_a, s->d_b + h, h, s->d_part + IP_BLOCKS + 1)) return e;
+        if (out_ip_l) ZK_CUDA(cudaMemcpyAsync(s->h_ip, s->d_part + IP_BLOCKS, 2 * sizeof(fe), cudaMemcpyDeviceToHost, ctx->stream));
+        return ipa_expand_and_msm<FS>(s, h, out_l_xyz, out_r_xyz);
+    });
     if (rc) return rc;
     if (out_ip_l) {
         ZK_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -187,15 +181,12 @@ int ipa_round_fold(zk_ipa* s, const uint64_t u_mont[4], const uint64_t u_inv_mon
     memcpy(u.v, u_mont, 32);
     memcpy(ui.v, u_inv_mont, 32);
     const unsigned blocks = (unsigned)((h + 127) / 128), sblocks = (unsigned)((count + 127) / 128);
-    if (s->curve == ZK_PALLAS) {
-        k_fold_field<FqParams><<<blocks, 128, 0, ctx->stream>>>(s->d_a, h, ui);
-        k_fold_field<FqParams><<<blocks, 128, 0, ctx->stream>>>(s->d_b, h, u);
-        k_expand_challenges<FqParams><<<sblocks, 128, 0, ctx->stream>>>(s->d_s[s->cur], s->d_s[s->cur ^ 1], count, u);
-    } else {
-        k_fold_field<FpParams><<<blocks, 128, 0, ctx->stream>>>(s->d_a, h, ui);
-        k_fold_field<FpParams><<<blocks, 128, 0, ctx->stream>>>(s->d_b, h, u);
-        k_expand_challenges<FpParams><<<sblocks, 128, 0, ctx->stream>>>(s->d_s[s->cur], s->d_s[s->cur ^ 1], count, u);
-    }
+    with_curve(s->curve, [&](auto c) {
+        using FS = typename decltype(c)::FS;
+        k_fold_field<FS><<<blocks, 128, 0, ctx->stream>>>(s->d_a, h, ui);
+        k_fold_field<FS><<<blocks, 128, 0, ctx->stream>>>(s->d_b, h, u);
+        k_expand_challenges<FS><<<sblocks, 128, 0, ctx->stream>>>(s->d_s[s->cur], s->d_s[s->cur ^ 1], count, u);
+    });
     ZK_CUDA(cudaGetLastError());
     ctx->launches += 3;
     s->cur ^= 1;
@@ -270,20 +261,21 @@ int zk_ipa_round_fold(zk_ipa* s, const uint64_t u_mont[4], const uint64_t u_inv_
 // against each other on the same machine (tools/fold_vs_never_fold.py, DESIGN.md 4.4) and is parity-tested like everything else.
 int zk_points_fold_dev(zk_ctx* ctx, int curve_id, const void* d_g, size_t h, const uint64_t u_mont[4], void* d_out) {
     if (!ctx || !u_mont || ((!d_g || !d_out) && h)) { zk_set_error("points_fold: null argument"); return ZK_ERR_INVALID; }
-    if (curve_id != ZK_PALLAS && curve_id != ZK_VESTA) { zk_set_error("points_fold: unknown curve_id %d", curve_id); return ZK_ERR_INVALID; }
+    if (int rc = check_curve("points_fold", curve_id)) return rc;
     std::lock_guard<std::mutex> lk(ctx->mu);
     ZK_CUDA(cudaSetDevice(ctx->device));
     if (h == 0) return ZK_OK;
     host::hfe um, unit = host::zero();
     memcpy(&um, u_mont, 32);
     unit.l[0] = 1;
-    // canonical u = u_mont / R: a Montgomery product with the integer 1
-    const host::hfe uc = curve_id == ZK_PALLAS ? host::mul<host::HFq>(um, unit) : host::mul<host::HFp>(um, unit);
-    fe k;
-    memcpy(&k, &uc, 32);
     const unsigned blocks = (unsigned)((h + 63) / 64);
-    if (curve_id == ZK_PALLAS) k_fold_bases<FpParams><<<blocks, 64, 0, ctx->stream>>>((const affine_t*)d_g, h, k, (affine_t*)d_out);
-    else k_fold_bases<FqParams><<<blocks, 64, 0, ctx->stream>>>((const affine_t*)d_g, h, k, (affine_t*)d_out);
+    with_curve(curve_id, [&](auto c) {
+        using C = decltype(c);
+        const host::hfe uc = host::mul<typename C::HS>(um, unit);     // canonical u = u_mont / R: a Montgomery product with the integer 1
+        fe k;
+        memcpy(&k, &uc, 32);
+        k_fold_bases<typename C::F><<<blocks, 64, 0, ctx->stream>>>((const affine_t*)d_g, h, k, (affine_t*)d_out);
+    });
     ZK_CUDA(cudaGetLastError());
     ctx->launches += 1;
     return ZK_OK;

@@ -16,7 +16,7 @@ struct zk_ipa {
     fe* d_a = nullptr;
     fe* d_b = nullptr;
     fe* d_part = nullptr;   // inner-product partials
-    fe* h_ip = nullptr;     // pinned (the context's scratch): two field elements
+    fe* h_ip = nullptr;     // the context's pinned PinnedSlots::ip: two field elements
     // SRS::open (open.cu): h and the fresh base U travel as extra points of every round's MSMs (ipa.rs:944,954), their scalars
     // (rand_l | rand_r of the round, and the round's two inner products) are appended on the device
     affine_t* d_extra = nullptr;   // [max(1, nwin)][2] rows of (h, U); null for the bare rounds of zk_ipa_*

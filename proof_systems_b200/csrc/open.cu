@@ -14,7 +14,6 @@
 #include <vector>
 
 #include "../../include/zkb200.h"
-#include "host_field.hpp"
 #include "ipa.hpp"
 #include "msm.cuh"
 #include "poly.cuh"
@@ -82,11 +81,12 @@ struct PtrKind {
     bool staged = false;
 };
 
-template <class F, class FS, class HP, class HS>
+template <class C>
 static int open_impl(zk_srs* srs, const zk_open_poly* polys, size_t n_polys, const uint64_t* elm_mont, size_t n_elm, const uint64_t polyscale[4],
                      const uint64_t evalscale[4], const uint64_t* rng, const zk_open_transcript* tr, uint64_t* out_lr_xy, unsigned rounds,
                      uint64_t out_delta_xy[8], uint64_t out_z1[4], uint64_t out_z2[4], uint64_t out_sg_xy[8]) {
     using namespace host;
+    using FS = typename C::FS; using HP = typename C::HP; using HS = typename C::HS;
     zk_ctx* ctx = srs->ctx;
     cudaStream_t st = ctx->stream;
     // ZKB200_TRACE_OPEN=1: wall-clock split of one call on stderr (diagnostic; tools/open_time.py)
@@ -95,7 +95,6 @@ static int open_impl(zk_srs* srs, const zk_open_poly* polys, size_t n_polys, con
     const auto t_begin = clk::now();
     auto ms_since = [](clk::time_point t0) { return std::chrono::duration<double, std::milli>(clk::now() - t0).count(); };
     double tr_lr = 0, tr_host = 0, tr_fold = 0;
-    const int scalar_field = srs->curve == ZK_PALLAS ? ZK_FQ : ZK_FP;
     const size_t srs_len = srs->n, n0 = (size_t)1 << rounds;
     const MsmBases& gb = srs->g->b;
     const unsigned c = gb.c, rows = c ? gb.nwin : 1;
@@ -123,20 +122,22 @@ static int open_impl(zk_srs* srs, const zk_open_poly* polys, size_t n_polys, con
             degree = p.domain_size;
         }
     }
-    // ---- device scratch: staged polynomial data | evaluation part | descriptors, elm, scales, blinders
+    // ---- device scratch: staged polynomial data, evaluation part, elm, scales, blinders | extra bases | descriptors
     unsigned log_deg = 0;
     while (((size_t)1 << log_deg) < degree) log_deg++;
     if (degree && log_deg > 30) { zk_set_error("open: evaluation domain too large"); return ZK_ERR_INVALID; }
     const size_t small_fe = n_elm * 2 + 2 * (size_t)rounds + 8;
     const size_t max_terms = n_polys + [&] { size_t t = 0; for (size_t k = 0; k < n_polys; k++) t += polys[k].n_blinders; return t; }();
-    const size_t bytes = (stage_elems + degree + small_fe) * sizeof(fe) + max_terms * sizeof(CombineDesc) + rows * 2 * sizeof(affine_t) + 256;
-    int rc = ctx_ensure((void**)&ctx->d_open, &ctx->cap_open, bytes);
+    Layout lay;
+    const size_t o_fe = lay.add((stage_elems + degree + small_fe) * sizeof(fe)), o_extra = lay.add(rows * 2 * sizeof(affine_t));
+    const size_t o_desc = lay.add(max_terms * sizeof(CombineDesc));
+    int rc = ctx->d_open.ensure(lay.total);
     if (rc) return rc;
-    fe* d_stage = (fe*)ctx->d_open;
+    fe* d_stage = ctx->d_open.at<fe>(o_fe);
     fe* d_evals = d_stage + stage_elems;
     fe* d_small = d_evals + degree;                       // elm | eval scales | rand_l, rand_r ...
-    affine_t* d_extra = (affine_t*)(d_small + small_fe);
-    CombineDesc* d_descs = (CombineDesc*)(d_extra + rows * 2);
+    affine_t* d_extra = ctx->d_open.at<affine_t>(o_extra);
+    CombineDesc* d_descs = ctx->d_open.at<CombineDesc>(o_desc);
     {
         size_t off = 0;
         for (size_t k = 0; k < n_polys; k++) {
@@ -177,9 +178,9 @@ static int open_impl(zk_srs* srs, const zk_open_poly* polys, size_t n_polys, con
     }
     // ---- the rounds' state: a and b are built in place
     zk_ipa* s = nullptr;
-    rc = ctx_ensure(&ctx->d_ipa, &ctx->cap_ipa, ipa_storage_bytes(n0));
+    rc = ctx->d_ipa.ensure(ipa_storage_bytes(n0));
     if (rc) return rc;
-    rc = ipa_create(ctx, srs->g, n0, &s, ctx->d_ipa);
+    rc = ipa_create(ctx, srs->g, n0, &s, ctx->d_ipa.p);
     if (rc) return rc;
     struct Guard { zk_ipa* s; ~Guard() { cudaStreamSynchronize(s->ctx->stream); ipa_release(s); } } guard{s};
     std::vector<CombineDesc> all_terms(coeff_terms);
@@ -190,7 +191,7 @@ static int open_impl(zk_srs* srs, const zk_open_poly* polys, size_t n_polys, con
     if (degree) {
         k_combine<FS><<<(unsigned)((degree + 127) / 128), 128, 0, st>>>(d_descs + coeff_terms.size(), (unsigned)eval_terms.size(), d_evals, degree);
         ZK_CUDA(cudaGetLastError());
-        rc = ctx_ntt_device(ctx, scalar_field, d_evals, log_deg, 1, 0, /*inverse=*/1, 0);     // Evaluations::interpolate (utils.rs:195-197)
+        rc = ctx_ntt_device(ctx, C::scalar_field, d_evals, log_deg, 1, 0, /*inverse=*/1, 0);     // Evaluations::interpolate (utils.rs:195-197)
         if (rc) return rc;
         const unsigned num_chunks = (unsigned)((degree + srs_len - 1) / srs_len);
         fe zeta;
@@ -316,9 +317,7 @@ extern "C" int zk_srs_open(zk_srs* srs, const zk_open_poly* polys, size_t n_poly
     zk_ctx* ctx = srs->ctx;
     std::lock_guard<std::mutex> lk(ctx->mu);   // held across the callbacks: they must not call into this context
     ZK_CUDA(cudaSetDevice(ctx->device));
-    if (srs->curve == ZK_PALLAS)
-        return open_impl<FpParams, FqParams, host::HFp, host::HFq>(srs, polys, n_polys, elm_mont, n_elm, polyscale, evalscale, rng_scalars, transcript,
-                                                                    out_lr_xy, rounds, out_delta_xy, out_z1, out_z2, out_sg_xy);
-    return open_impl<FqParams, FpParams, host::HFq, host::HFp>(srs, polys, n_polys, elm_mont, n_elm, polyscale, evalscale, rng_scalars, transcript,
-                                                                out_lr_xy, rounds, out_delta_xy, out_z1, out_z2, out_sg_xy);
+    return with_curve(srs->curve, [&](auto c) {
+        return open_impl<decltype(c)>(srs, polys, n_polys, elm_mont, n_elm, polyscale, evalscale, rng_scalars, transcript, out_lr_xy, rounds, out_delta_xy, out_z1, out_z2, out_sg_xy);
+    });
 }

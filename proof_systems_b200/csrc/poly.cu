@@ -44,13 +44,12 @@ extern "C" {
 
 int zk_poly_add_dev(zk_ctx* ctx, int field_id, void* d_dst, const void* d_src, size_t len) {
     if (!ctx || ((!d_dst || !d_src) && len)) { zk_set_error("poly_add: null argument"); return ZK_ERR_INVALID; }
-    if (field_id != ZK_FP && field_id != ZK_FQ) { zk_set_error("poly_add: unknown field_id %d", field_id); return ZK_ERR_INVALID; }
+    if (int rc = check_field("poly_add", field_id)) return rc;
     std::lock_guard<std::mutex> lk(ctx->mu);
     ZK_CUDA(cudaSetDevice(ctx->device));
     if (len == 0) return ZK_OK;
     const unsigned blocks = (unsigned)((len + 255) / 256);
-    if (field_id == ZK_FP) k_vec_add<FpParams><<<blocks, 256, 0, ctx->stream>>>((fe*)d_dst, (const fe*)d_src, len);
-    else k_vec_add<FqParams><<<blocks, 256, 0, ctx->stream>>>((fe*)d_dst, (const fe*)d_src, len);
+    with_field(field_id, [&](auto f) { k_vec_add<typename decltype(f)::Dev><<<blocks, 256, 0, ctx->stream>>>((fe*)d_dst, (const fe*)d_src, len); });
     ZK_CUDA(cudaGetLastError());
     ctx->launches += 1;
     return ZK_OK;
@@ -58,24 +57,24 @@ int zk_poly_add_dev(zk_ctx* ctx, int field_id, void* d_dst, const void* d_src, s
 
 int zk_poly_divide_by_vanishing_dev(zk_ctx* ctx, int field_id, const void* d_f, size_t len, unsigned log_n, void* d_quot, int* remainder_is_zero) {
     if (!ctx || !d_f || !remainder_is_zero) { zk_set_error("divide_by_vanishing: null argument"); return ZK_ERR_INVALID; }
-    if (field_id != ZK_FP && field_id != ZK_FQ) { zk_set_error("divide_by_vanishing: unknown field_id %d", field_id); return ZK_ERR_INVALID; }
-    if (log_n > 30) { zk_set_error("divide_by_vanishing: log_n %u > 30", log_n); return ZK_ERR_INVALID; }
+    if (int rc = check_field("divide_by_vanishing", field_id)) return rc;
+    if (int rc = check_log_n("divide_by_vanishing", log_n)) return rc;
     const size_t n = (size_t)1 << log_n;
     if (len > n && !d_quot) { zk_set_error("divide_by_vanishing: null quotient buffer"); return ZK_ERR_INVALID; }
     std::lock_guard<std::mutex> lk(ctx->mu);
     ZK_CUDA(cudaSetDevice(ctx->device));
-    if (!ctx->h_scratch) ZK_CUDA(cudaMallocHost(&ctx->h_scratch, 256));
-    if (!ctx->d_flag) ZK_CUDA(cudaMalloc(&ctx->d_flag, sizeof(unsigned)));
-    ZK_CUDA(cudaMemsetAsync(ctx->d_flag, 0, sizeof(unsigned), ctx->stream));
+    PinnedSlots* pin = ctx_pinned(ctx);
+    if (!pin) return ZK_ERR_CUDA;
+    if (int rc = ctx->d_flag.ensure(sizeof(unsigned))) return rc;
+    unsigned* d_flag = ctx->d_flag.at<unsigned>();
+    ZK_CUDA(cudaMemsetAsync(d_flag, 0, sizeof(unsigned), ctx->stream));
     const unsigned blocks = (unsigned)((n + 127) / 128);
-    if (field_id == ZK_FP) k_divide_by_vanishing<FpParams><<<blocks, 128, 0, ctx->stream>>>((const fe*)d_f, len, n, (fe*)d_quot, ctx->d_flag);
-    else k_divide_by_vanishing<FqParams><<<blocks, 128, 0, ctx->stream>>>((const fe*)d_f, len, n, (fe*)d_quot, ctx->d_flag);
+    with_field(field_id, [&](auto f) { k_divide_by_vanishing<typename decltype(f)::Dev><<<blocks, 128, 0, ctx->stream>>>((const fe*)d_f, len, n, (fe*)d_quot, d_flag); });
     ZK_CUDA(cudaGetLastError());
     ctx->launches += 1;
-    unsigned* h = (unsigned*)((char*)ctx->h_scratch + 192);
-    ZK_CUDA(cudaMemcpyAsync(h, ctx->d_flag, sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));
+    ZK_CUDA(cudaMemcpyAsync(&pin->remainder, d_flag, sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));
     ZK_CUDA(cudaStreamSynchronize(ctx->stream));
-    *remainder_is_zero = *h == 0;
+    *remainder_is_zero = pin->remainder == 0;
     return ZK_OK;
 }
 

@@ -53,16 +53,14 @@ template <class FS> __global__ void __launch_bounds__(128) k_perm_quotient(const
     store_fe(a.out + i, r);
 }
 
-int ctx_ntt_table_ptrs(zk_ctx* ctx, int field, unsigned log_n, bool inverse, const fe** ulo, const fe** mid, const fe** hi2);   // api.cu
-
 }  // namespace zkb
 
 extern "C" int zk_perm_quotient_dev(zk_ctx* ctx, int field_id, unsigned log_m, const void* const d_w[7], const void* d_z, const void* const d_sigma[7],
                                     const void* d_zkpm, const uint64_t beta[4], const uint64_t gamma[4], const uint64_t alpha0[4],
                                     const uint64_t shifts[28], unsigned next_shift, void* d_out) {
     if (!ctx || !d_w || !d_z || !d_sigma || !d_zkpm || !beta || !gamma || !alpha0 || !shifts || !d_out) { zk_set_error("perm_quotient: null argument"); return ZK_ERR_INVALID; }
-    if (field_id != ZK_FP && field_id != ZK_FQ) { zk_set_error("perm_quotient: unknown field_id %d", field_id); return ZK_ERR_INVALID; }
-    if (log_m > 30) { zk_set_error("perm_quotient: log_m %u > 30", log_m); return ZK_ERR_INVALID; }
+    if (int rc = check_field("perm_quotient", field_id)) return rc;
+    if (int rc = check_log_n("perm_quotient", log_m, "log_m")) return rc;
     const size_t m = (size_t)1 << log_m;
     if (next_shift >= m) { zk_set_error("perm_quotient: shift %u does not fit a domain of %zu", next_shift, m); return ZK_ERR_INVALID; }
     for (int k = 0; k < 7; k++)
@@ -78,8 +76,7 @@ extern "C" int zk_perm_quotient_dev(zk_ctx* ctx, int field_id, unsigned log_m, c
     memcpy(&a.beta, beta, 32); memcpy(&a.gamma, gamma, 32); memcpy(&a.alpha0, alpha0, 32);
     memcpy(a.shift, shifts, 7 * 32);
     const unsigned blocks = (unsigned)((m + 127) / 128);
-    if (field_id == ZK_FP) k_perm_quotient<FpParams><<<blocks, 128, 0, ctx->stream>>>(a);
-    else k_perm_quotient<FqParams><<<blocks, 128, 0, ctx->stream>>>(a);
+    with_field(field_id, [&](auto f) { k_perm_quotient<typename decltype(f)::Dev><<<blocks, 128, 0, ctx->stream>>>(a); });
     ZK_CUDA(cudaGetLastError());
     ctx->launches += 1;
     return ZK_OK;

@@ -13,7 +13,6 @@
 
 #include "../../include/zkb200.h"
 #include "ctx.hpp"
-#include "host_field.hpp"
 #include "msm.cuh"
 
 using namespace zkb;
@@ -88,24 +87,24 @@ int zk_srs_lagrange_basis(zk_srs* srs, size_t domain_size, int window_bits) {
     while (((size_t)1 << log_n) < domain_size) log_n++;
     const size_t chunks = basis_chunks(srs, domain_size);
     zk_ctx* ctx = srs->ctx;
-    affine_t* d_out = nullptr;
-    int rc = ZK_OK;
+    DevScratch d_out;                    // transient: freed on every return
     {
         std::lock_guard<std::mutex> lk(ctx->mu);
         ZK_CUDA(cudaSetDevice(ctx->device));
-        ZK_CUDA(cudaMalloc(&d_out, chunks * domain_size * sizeof(affine_t)));
+        if (int rc = d_out.ensure(chunks * domain_size * sizeof(affine_t))) return rc;
         unsigned nl = 0;
+        int rc = ZK_OK;
         for (size_t c = 0; c < chunks && rc == ZK_OK; c++)
-            rc = srs->curve == ZK_PALLAS ? lagrange_basis_build<FpParams, FqParams>(srs->g->b, log_n, (unsigned)c, d_out + c * domain_size, ctx->stream, &nl)
-                                         : lagrange_basis_build<FqParams, FpParams>(srs->g->b, log_n, (unsigned)c, d_out + c * domain_size, ctx->stream, &nl);
+            rc = with_curve(srs->curve, [&](auto cv) {
+                using C = decltype(cv);
+                return lagrange_basis_build<typename C::F, typename C::FS>(srs->g->b, log_n, (unsigned)c, d_out.at<affine_t>() + c * domain_size, ctx->stream, &nl);
+            });
         ctx->launches += nl;
+        if (rc) return rc;
     }
-    if (rc == ZK_OK) {
-        zk_bases* b = nullptr;
-        rc = zk_bases_upload(ctx, srs->curve, (const uint64_t*)d_out, chunks * domain_size, window_bits, /*points_on_device=*/1, &b);
-        if (rc == ZK_OK) srs->lagrange.emplace(domain_size, b);
-    }
-    cudaFree(d_out);
+    zk_bases* b = nullptr;
+    int rc = zk_bases_upload(ctx, srs->curve, d_out.at<const uint64_t>(), chunks * domain_size, window_bits, /*points_on_device=*/1, &b);
+    if (rc == ZK_OK) srs->lagrange.emplace(domain_size, b);
     return rc;
 }
 
@@ -219,10 +218,8 @@ int zk_srs_mask_custom(zk_srs* srs, const uint64_t* chunks_xy, size_t n_chunks, 
         zk_set_error("BlindersDontMatch(%zu, %zu)", n_blinders, n_chunks);  // poly-commitment/src/error.rs:3-9
         return ZK_ERR_LENGTH;
     }
-    for (size_t i = 0; i < n_chunks; i++) {
-        if (srs->curve == ZK_PALLAS) mask_one<host::HFp, host::HFq>(chunks_xy + 8 * i, blinders_mont + 4 * i, srs->h, out_xy + 8 * i);
-        else mask_one<host::HFq, host::HFp>(chunks_xy + 8 * i, blinders_mont + 4 * i, srs->h, out_xy + 8 * i);
-    }
+    for (size_t i = 0; i < n_chunks; i++)
+        with_curve(srs->curve, [&](auto c) { mask_one<typename decltype(c)::HP, typename decltype(c)::HS>(chunks_xy + 8 * i, blinders_mont + 4 * i, srs->h, out_xy + 8 * i); });
     return ZK_OK;
 }
 

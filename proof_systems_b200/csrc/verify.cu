@@ -20,7 +20,6 @@
 
 #include "../../include/zkb200.h"
 #include "ctx.hpp"
-#include "host_field.hpp"
 #include "msm.cuh"
 
 using namespace zkb;
@@ -65,9 +64,10 @@ __global__ void k_verify_s(const fe* __restrict__ lo, const fe* __restrict__ hi,
     store_fe(S + j, acc);
 }
 
-template <class F, class FS, class HP, class HS>
+template <class C>
 static int verify_impl(zk_srs* srs, const zk_verify_proof* batch, size_t B, const uint64_t* rng, int* out_ok, uint64_t* out_sum_xyz) {
     using namespace host;
+    using FS = typename C::FS; using HP = typename C::HP; using HS = typename C::HS;
     zk_ctx* ctx = srs->ctx;
     cudaStream_t st = ctx->stream;
     // ZKB200_TRACE_VERIFY=1: wall-clock split of one call on stderr (diagnostic; tools/verify_time.py)
@@ -176,19 +176,19 @@ static int verify_impl(zk_srs* srs, const zk_verify_proof* batch, size_t B, cons
     sc[0] = h_scalar;
     const auto t_host = clk::now();
 
-    // ---- device scratch: S | lo tables | hi tables | rev | weights | proof scalars | proof points (affine, 64-byte aligned)
+    // ---- device scratch: S, lo tables, hi tables, rev, weights, proof scalars | proof points (affine)
     const size_t n_lo = (size_t)B << L, n_hi = (size_t)B << H;
-    const size_t n_fe = len + n_lo + n_hi + rev.size() + B + n_pts;
-    const size_t bytes = ((n_fe * sizeof(fe) + 63) & ~(size_t)63) + n_pts * sizeof(affine_t);
-    int rc = ctx_ensure(&ctx->d_verify, &ctx->cap_verify, bytes);
+    Layout lay;
+    const size_t o_fe = lay.add((len + n_lo + n_hi + rev.size() + B + n_pts) * sizeof(fe)), o_pts = lay.add(n_pts * sizeof(affine_t));
+    int rc = ctx->d_verify.ensure(lay.total);
     if (rc) return rc;
-    fe* d_S = (fe*)ctx->d_verify;
+    fe* d_S = ctx->d_verify.at<fe>(o_fe);
     fe* d_lo = d_S + len;
     fe* d_hi = d_lo + n_lo;
     fe* d_rev = d_hi + n_hi;
     fe* d_w = d_rev + rev.size();
     fe* d_sc = d_w + B;
-    affine_t* d_pts = (affine_t*)((char*)ctx->d_verify + ((n_fe * sizeof(fe) + 63) & ~(size_t)63));
+    affine_t* d_pts = ctx->d_verify.at<affine_t>(o_pts);
     ZK_CUDA(cudaMemcpyAsync(d_rev, rev.data(), rev.size() * sizeof(fe), cudaMemcpyHostToDevice, st));
     ZK_CUDA(cudaMemcpyAsync(d_w, wts.data(), B * sizeof(fe), cudaMemcpyHostToDevice, st));
     ZK_CUDA(cudaMemcpyAsync(d_sc, sc.data(), n_pts * sizeof(fe), cudaMemcpyHostToDevice, st));
@@ -256,7 +256,7 @@ extern "C" int zk_srs_verify(zk_srs* srs, const zk_verify_proof* batch, size_t n
     if (n == 0) {                 // the reference's MSM of all-zero scalars is the identity
         *out_ok = 1;
         if (out_sum_xyz) {
-            const host::hjac id = srs->curve == ZK_PALLAS ? host::to_jacobian<host::HFp>(host::identity()) : host::to_jacobian<host::HFq>(host::identity());
+            const host::hjac id = with_curve(srs->curve, [](auto c) { return host::to_jacobian<typename decltype(c)::HP>(host::identity()); });
             memcpy(out_sum_xyz, &id, 96);
         }
         return ZK_OK;
@@ -264,6 +264,5 @@ extern "C" int zk_srs_verify(zk_srs* srs, const zk_verify_proof* batch, size_t n
     zk_ctx* ctx = srs->ctx;
     std::lock_guard<std::mutex> lk(ctx->mu);   // held across the callbacks: they must not call into this context
     ZK_CUDA(cudaSetDevice(ctx->device));
-    if (srs->curve == ZK_PALLAS) return verify_impl<FpParams, FqParams, host::HFp, host::HFq>(srs, batch, n, rng_scalars, out_ok, out_sum_xyz);
-    return verify_impl<FqParams, FpParams, host::HFq, host::HFp>(srs, batch, n, rng_scalars, out_ok, out_sum_xyz);
+    return with_curve(srs->curve, [&](auto c) { return verify_impl<decltype(c)>(srs, batch, n, rng_scalars, out_ok, out_sum_xyz); });
 }
