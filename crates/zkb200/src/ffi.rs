@@ -158,6 +158,9 @@ extern "C" {
     pub fn zk_prover_ft_dev(ctx: *mut zk_ctx, field_id: c_int, log_n: c_uint, max_poly_size: usize, terms: *const zk_lin_term, n_terms: usize,
                             d_t: *const c_void, t_len: usize, zeta_mont: *const u64, d_ft: *mut c_void, ft_len: *mut usize,
                             ft_eval1: *mut u64) -> c_int;
+    pub fn zk_perm_aggreg_dev(ctx: *mut zk_ctx, field_id: c_int, log_n: c_uint, zk_rows: usize, d_w: *const *const c_void,
+                              d_sigma: *const *const c_void, sigma_len: u64, beta: *const u64, gamma: *const u64, shifts: *const u64,
+                              rand: *const u64, d_z: *mut c_void, final_is_one: *mut c_int) -> c_int;
 
     pub fn zk_ntt_batch(ctx: *mut zk_ctx, field_id: c_int, data: *mut u64, log_n: c_uint, batch: usize, in_len: usize, inverse: c_int,
                         coset: c_int) -> c_int;

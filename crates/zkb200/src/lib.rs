@@ -13,6 +13,8 @@
 //!   (kimchi/src/prover.rs:1009-1058) over the same resident columns (`zk_lagrange_evaluate_dev`, `zk_poly_evaluate_chunks_dev`).
 //! * [`ft::ft_dev`] computes the ft polynomial of Maller's optimisation (kimchi/src/prover.rs:1147-1206) from the resident quotient
 //!   and sigma_6 over d8, leaving ft resident for the opening proof (`zk_prover_ft_dev`).
+//! * [`perm::perm_aggreg_dev`] builds the permutation aggregation polynomial z (kimchi/src/circuits/polynomials/permutation.rs:447-574)
+//!   from the resident witness and `permutation_coefficients8`, leaving z resident (`zk_perm_aggreg_dev`).
 //!
 //! Everything called is declared in include/zkb200.h and exported by libzkb200.so; there is no CPU fallback inside the library
 //! (`Ctx::new` fails without a CUDA device) — code that must also run without a GPU keeps using `ipa::SRS`.
@@ -23,6 +25,7 @@ pub mod ffi;
 pub mod ft;
 pub mod marshal;
 pub mod open;
+pub mod perm;
 pub mod srs;
 
 pub use domain::GpuRadix2Domain;

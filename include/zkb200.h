@@ -327,6 +327,23 @@ int zk_perm_quotient_dev(zk_ctx* ctx, int field_id, unsigned log_m, const void* 
                          const void* const d_sigma[7], const void* d_zkpm, const uint64_t beta[4], const uint64_t gamma[4],
                          const uint64_t alpha0[4], const uint64_t shifts[28], unsigned next_shift, void* d_out);
 
+/* ------------------------------------------------------------------ permutation aggregation polynomial z
+ * ProverIndex::perm_aggreg (kimchi/src/circuits/polynomials/permutation.rs:447-574) over resident operands.  With n = 2^log_n,
+ * last = n - zk_rows, sid[j] = omega^j and s = sigma_len / n:
+ *   num[j] = prod_{k<7} (w_k[j] + sid[j] beta shift_k + gamma),   den[j] = prod_{k<7} (w_k[j] + sigma_k[s j] beta + gamma)
+ *   z[0] = 1;  z[j + 1] = z[j] num[j] / den[j] for j < n - 1, except z[last + 1] = rand[0..3] and z[last + 2] = rand[4..7]
+ * A zero den[j] is inverted to zero (ark_ff::batch_inversion skips it), so z is zero from row j + 1 on, up to the random rows.
+ * d_w[k]: n evaluations of witness column k over d1; d_sigma[k]: sigma_len evaluations (n <= sigma_len <= 8n, a multiple of n:
+ * kimchi's permutation_coefficients8, 8n, e.g. a cached index's sections 0x30 .. 0x36); beta, gamma, the 7 shifts (cs.shift) and
+ * the caller's two F::rand(rng) draws, in the reference's order: Montgomery and canonical.  d_z receives z's n coefficients
+ * (Evaluations::interpolate, untrimmed; it may not overlap an input) and *final_is_one whether z[last] == 1 — the reference returns
+ * ProverError::Permutation("final value") when it is not; z is written either way.  Runs on the context's stream and synchronises once.
+ * Errors, before anything runs (d_z is untouched): ZK_ERR_INVALID for a null pointer, an unknown field, log_n > 30, zk_rows < 3
+ * or zk_rows >= n, a sigma_len that is not 1 .. 8 times n, a scalar that is not a canonical field element, d_z overlapping an input. */
+int zk_perm_aggreg_dev(zk_ctx* ctx, int field_id, unsigned log_n, size_t zk_rows, const void* const d_w[7], const void* const d_sigma[7],
+                       uint64_t sigma_len, const uint64_t beta[4], const uint64_t gamma[4], const uint64_t shifts[28], const uint64_t rand[8],
+                       void* d_z, int* final_is_one);
+
 /* ------------------------------------------------------------------ constraint evaluator (kimchi's expression framework)
  * zk_expr_eval_dev replaces Expr::evaluations(&env) (kimchi/src/circuits/expr.rs:1938-2190; call sites kimchi/src/prover.rs:794-892:
  * every gate's combined constraint and the lookup constraints, evaluated over d4 or d8 and added into t4 / t8).  The expression is

@@ -131,6 +131,7 @@ def lib() -> ctypes.CDLL:
     L.zk_lagrange_evaluate_dev.argtypes = [vp, i, ctypes.POINTER(vp), sz, u, sz, ctypes.POINTER(EvalColumn), sz, vp]
     L.zk_poly_evaluate_chunks_dev.argtypes = [vp, i, ctypes.POINTER(DevPoly), sz, sz, sz, vp, sz, vp]
     L.zk_prover_ft_dev.argtypes = [vp, i, u, sz, ctypes.POINTER(LinTerm), sz, vp, sz, vp, vp, ctypes.POINTER(sz), vp]
+    L.zk_perm_aggreg_dev.argtypes = [vp, i, u, sz, ctypes.POINTER(vp), ctypes.POINTER(vp), ctypes.c_uint64, vp, vp, vp, vp, vp, ctypes.POINTER(i)]
     return L
 
 
@@ -460,6 +461,21 @@ class Context:
         check(lib().zk_prover_ft_dev(self._h, field, log_n, max_poly_size, arr, len(terms), ctypes.c_void_p(d_t), t_len, _ptr(zv),
                                      ctypes.c_void_p(d_ft), ctypes.byref(ft_len), _ptr(ev1)))
         return int(ft_len.value), ev1
+
+    # ------------------------------------------------------------------ permutation aggregation polynomial z (zk_perm_aggreg_dev)
+    def perm_aggreg_dev(self, field: int, log_n: int, zk_rows: int, d_w, d_sigma, sigma_len: int, beta, gamma, shifts, rand, d_z: int) -> bool:
+        """zk_perm_aggreg_dev (kimchi's ProverIndex::perm_aggreg): z's 2^log_n coefficients into d_z from the 7 resident witness columns
+        d_w (2^log_n evaluations each) and the 7 resident sigma columns d_sigma (sigma_len evaluations each, read at stride
+        sigma_len / 2^log_n); beta, gamma [4], shifts [7, 4] and rand [2, 4] (the two F::rand draws) Montgomery.  Returns whether
+        z[n - zk_rows] == 1 (the reference's "final value" check); z is written either way."""
+        c = lambda a, k: np.ascontiguousarray(a, dtype=np.uint64).reshape(k)
+        b, g, sh, rn = c(beta, 4), c(gamma, 4), c(shifts, 28), c(rand, 8)
+        pw = (ctypes.c_void_p * 7)(*[int(p) for p in d_w])
+        ps = (ctypes.c_void_p * 7)(*[int(p) for p in d_sigma])
+        ok = ctypes.c_int()
+        check(lib().zk_perm_aggreg_dev(self._h, field, log_n, zk_rows, pw, ps, sigma_len, _ptr(b), _ptr(g), _ptr(sh), _ptr(rn),
+                                       ctypes.c_void_p(d_z), ctypes.byref(ok)))
+        return bool(ok.value)
 
     def points_fold_dev(self, curve: int, d_g: int, h: int, u_mont, d_out: int):
         """zk_points_fold_dev: out[i] = g[i] + [u] g[h + i] on device-resident affine points (the reference's per-round base fold)"""

@@ -88,6 +88,7 @@ struct PinnedSlots {
     unsigned remainder;         // zk_poly_divide_by_vanishing_dev: nonzero remainder flag
     unsigned long long ft_len;  // zk_prover_ft_dev: ft's length and ft(zeta omega)
     fe ft_eval1;
+    unsigned perm_final;        // zk_perm_aggreg_dev: z[n - zk_rows] == 1
 };
 }  // namespace zkb
 
@@ -127,6 +128,7 @@ struct zk_ctx {
     zkb::DevScratch d_verify;            // zk_srs_verify: s vector | challenge tables | proof points and their scalars
     zkb::DevScratch d_evals;             // zk_lagrange_evaluate_dev / zk_poly_evaluate_chunks_dev: descriptors | partial sums | results
     zkb::DevScratch d_ft;                // zk_prover_ft_dev: f over d1 | term descriptors | length counter
+    zkb::DevScratch d_perm;              // zk_perm_aggreg_dev: den, then num / den over d1 | block products | final-value flag
     uint64_t launches = 0;
     bool profile = false;                // per-stage device timing (zk_ctx_set_profile)
     cudaEvent_t ev_ntt[2] = {nullptr, nullptr};
