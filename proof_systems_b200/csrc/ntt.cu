@@ -49,7 +49,7 @@ template <class F> __global__ void k_full_table(fe* full, const fe* __restrict__
     const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= n) return;
     const unsigned k = (unsigned)(idx & (((size_t)1 << log_n1) - 1)), col = (unsigned)(idx >> log_n1);
-    const unsigned e = col * k;          // < n <= 2^22
+    const unsigned e = col * k;          // < n <= 2^20
     fe tw = load_fe_nc(lo + (e & 1023));
     if (e >> 10) tw = fe_mul<F>(tw, load_fe_nc(mid + (e >> 10)));
     store_fe(full + idx, tw);
@@ -80,7 +80,7 @@ template <class F> int ntt_build_tables(NttTables& t, unsigned log_n, bool inver
     k_pow_table<F><<<4, 256, 0, st>>>(t.clo, bases + 2, bases + 5, 1024);  // g^i
     k_pow_table<F><<<4, 256, 0, st>>>(t.chi, bases + 3, bases + 5, 1024);  // g^(1024 i)
     t.full = nullptr;
-    if (log_n > NTT_MAX_LOG_SUB && log_n <= NTT_FULL_TABLE_MAX_LOG) {
+    if (log_n > NTT_MAX_LOG_SUB && log_n <= 2 * NTT_MAX_LOG_SUB) {     // only the two-pass plan reads it (ntt_run)
         const size_t n = (size_t)1 << log_n;
         const unsigned log_n1 = (log_n + 1) / 2;
         ZK_CUDA(cudaMalloc(&t.full, n * sizeof(fe)));

@@ -15,7 +15,8 @@
 // layers of span <= 32 for a 64-row chunk entirely in REGISTERS (two elements per lane, partners exchanged with warp shuffles,
 // one multiplication per lane and layer: ntt_butterfly.cuh), the remaining log2(S) - 6 layers go through shared memory
 // (limb-major, padded: conflict-free), and the store — natural order, no permutation left — fuses the inter-pass twiddle
-// (one multiplication against an n-entry table kept in HBM for n <= 2^22, or two against 1024-entry tables), the 1/n scaling
+// (one multiplication against an n-entry table kept in HBM for the two-pass plan, n <= 2^20, or up to two against 1024-entry
+// tables in the three-pass plan), the 1/n scaling
 // (folded into the tables) and the transposition.  Work is 255-bit modular integer arithmetic: no tensor cores.
 #pragma once
 #include "common.cuh"
@@ -24,7 +25,6 @@ namespace zkb {
 
 constexpr unsigned NTT_MAX_LOG_SUB = 10;   // sub-transform size limit (one column per tile, twiddles from a 512-entry table)
 constexpr unsigned NTT_MAX_LOG_N = 30;     // three passes of <= 2^10
-constexpr unsigned NTT_FULL_TABLE_MAX_LOG = 22;   // n-entry inter-pass twiddle table up to this size (128 MiB)
 
 // device tables of one (field, log_n, direction)
 struct NttTables {
@@ -34,7 +34,7 @@ struct NttTables {
     fe* hi2 = nullptr;   // [1024] w_n^(+-2^20 i)
     fe* clo = nullptr;   // [1024] g^(+-i)              coset powers
     fe* chi = nullptr;   // [1024] g^(+-1024 i)
-    fe* full = nullptr;  // [n]    w_n^(+-(col * k)) (inverse: times n^-1) at index col * n1 + k: contiguous per tile of pass 1; or null
+    fe* full = nullptr;  // [n]    w_n^(+-(col * k)) (inverse: times n^-1) at index col * n1 + k: contiguous per tile of pass 1; null outside 2^10 < n <= 2^20
 };
 
 // One pass = independent S-point transforms of columns ("tiles").  Tile tau = (t_hi << split_log) | t_lo of polynomial b reads

@@ -17,7 +17,7 @@ def ctx():
     c.close()
 
 
-@pytest.mark.parametrize("fid,log_m", [(0, 10), (1, 13)])
+@pytest.mark.parametrize("fid,log_m", [(0, 10), (1, 13), (0, 21), (1, 22)])
 def test_permutation_quotient_kernel_vs_oracle(ctx, orc, fid, log_m):
     m = 1 << log_m
     rnd = lambda k, seed: orc.to_mont(fid, orc.random_scalars(fid, k, seed=seed))

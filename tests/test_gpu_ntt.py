@@ -147,10 +147,11 @@ def test_pinned_host_memory_is_transformed_in_place(ctx, orc):
             assert np.array_equal(view[j], orc.ntt(zk.FQ, a[j], inverse=True)), (log_n, j)
 
 
-@pytest.mark.parametrize("fid,log_n", [(0, 21), (1, 22)])
+@pytest.mark.parametrize("fid,log_n", [(0, 21), (1, 22), (0, 23), (1, 24), (0, 25)])
 def test_three_pass_plan_beyond_2_20(ctx, orc, fid, log_n):
     """kimchi's d8 for a 2^18-gate circuit is 2^21 (kimchi/src/circuits/domains.rs:40-69): transforms beyond 2^20 run as three
-    passes (n = n1 n2 n3).  Forward vs the oracle, inverse(forward) == input, and the zero-padded form."""
+    passes (n = n1 n2 n3; log2 of the factors 7.7.7, 8.7.7, 8.8.7, 8.8.8 and 9.8.8 from 2^21 to 2^25).  Forward vs the oracle,
+    inverse(forward) == input, and the zero-padded form."""
     n = 1 << log_n
     a = orc.to_mont(fid, orc.random_scalars(fid, n, seed=80 + log_n))
     f = ctx.ntt(fid, a)
