@@ -55,7 +55,11 @@ const char* zk_last_error(void);
 int zk_device_count(void);
 int zk_ctx_create(int device_id, zk_ctx** out);
 void zk_ctx_destroy(zk_ctx* ctx);
-/* Run on the caller's CUDA stream (a cudaStream_t, e.g. torch.cuda.current_stream().cuda_stream); NULL = own stream. */
+/* Run on the caller's CUDA stream (a cudaStream_t); NULL = the context's own stream, which is non-blocking and so NOT ordered
+ * with the legacy default stream.  To run on the legacy default stream pass cudaStreamLegacy, never 0: torch's default stream
+ * has the handle 0 (torch.cuda.current_stream().cuda_stream), and passing it unchanged selects the own stream instead.  When
+ * the stream changes, the new one waits (on the device) for all work the context queued on the old one.  Calls that return
+ * with work still queued keep it on the stream that was current; the caller orders its own reads after them on that stream. */
 int zk_ctx_set_stream(zk_ctx* ctx, void* cuda_stream);
 /* Kernels launched by this context so far (bench.py's gpu_launches). */
 uint64_t zk_ctx_launch_count(const zk_ctx* ctx);

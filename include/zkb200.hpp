@@ -51,6 +51,7 @@ class Context {
     Context(const Context&) = delete;
     Context& operator=(const Context&) = delete;
     zk_ctx* handle() const { return h_; }
+    // nullptr = the context's own (non-blocking) stream; for the legacy default stream pass cudaStreamLegacy, not 0 (zkb200.h)
     void set_stream(void* cuda_stream) { check(zk_ctx_set_stream(h_, cuda_stream)); }
     void set_option(const char* name, long value) { check(zk_ctx_set_option(h_, name, value)); }
     uint64_t launch_count() const { return zk_ctx_launch_count(h_); }

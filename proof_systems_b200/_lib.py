@@ -10,6 +10,7 @@ FP, FQ = 0, 1
 PALLAS, VESTA = 0, 1
 BASE_FIELD = {PALLAS: FP, VESTA: FQ}
 SCALAR_FIELD = {PALLAS: FQ, VESTA: FP}
+CUDA_STREAM_LEGACY = 0x1             # cudaStreamLegacy (cuda_runtime_api.h)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # ZKB200_LIB: an alternative BUILD of the same CUDA library (tools/mul_variants.sh times the field-product variants
@@ -249,7 +250,10 @@ class Context:
             pass
 
     def set_stream(self, cuda_stream: int | None):
-        check(lib().zk_ctx_set_stream(self._h, ctypes.c_void_p(cuda_stream or 0)))
+        """None: the library's own stream.  An integer is a cudaStream_t handle, 0 included: 0 is the legacy default stream (torch's
+        default stream reports 0 as its cuda_stream) and reaches the C ABI as cudaStreamLegacy, whose NULL means the own stream."""
+        handle = None if cuda_stream is None else (int(cuda_stream) or CUDA_STREAM_LEGACY)
+        check(lib().zk_ctx_set_stream(self._h, ctypes.c_void_p(handle)))
 
     @property
     def launch_count(self) -> int:

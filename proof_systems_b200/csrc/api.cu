@@ -186,13 +186,21 @@ static int ctx_init_lane(zk_ctx* c, int device_id) {
     return ZK_OK;
 }
 
+// host-pointer calls share the lane pool only on the own stream, unprofiled, with more than one lane (ctx->mu held)
+static void ctx_update_pinned(zk_ctx* ctx) { ctx->pinned = ctx->stream != ctx->own_stream || ctx->profile || ctx->n_lanes <= 1; }
+
 int ctx_acquire_lane(zk_ctx* ctx, LaneLock& out) {
     ctx = ctx_root(ctx);
-    const bool pinned = ctx->stream != ctx->own_stream || ctx->profile || ctx->n_lanes <= 1;
-    if (pinned) {
-        out.lane = ctx;
-        out.lk = std::unique_lock<std::mutex>(ctx->mu);
-        return ZK_OK;
+    {
+        // a free primary lane is taken whether or not calls are pinned to it; a busy one is waited for only when they are (a
+        // blocking lock here would serialise the pool)
+        std::unique_lock<std::mutex> root_lk(ctx->mu, std::try_to_lock);
+        if (root_lk.owns_lock() || ctx->pinned.load()) {
+            if (!root_lk.owns_lock()) root_lk.lock();
+            out.lane = ctx;
+            out.lk = std::move(root_lk);
+            return ZK_OK;
+        }
     }
     std::vector<zk_ctx*> lanes;
     unsigned start;
@@ -318,6 +326,7 @@ void zk_ctx_destroy(zk_ctx* ctx) {
     for (int l = 0; l < zk_ctx::SIDE_STREAMS; l++)
         if (ctx->side[l]) { cudaStreamSynchronize(ctx->side[l]); cudaStreamDestroy(ctx->side[l]); }
     if (ctx->ev_fork) cudaEventDestroy(ctx->ev_fork);
+    if (ctx->ev_switch) cudaEventDestroy(ctx->ev_switch);
     for (int f = 0; f < 2; f++) for (int d = 0; d < 2; d++) if (ctx->ntt_small[f][d]) cudaFree(ctx->ntt_small[f][d]);
     for (auto& kv : ctx->ntt_tables) ntt_free_tables(kv.second);
     for (auto& e : ctx->ev_ntt) if (e) cudaEventDestroy(e);
@@ -328,7 +337,16 @@ void zk_ctx_destroy(zk_ctx* ctx) {
 int zk_ctx_set_stream(zk_ctx* ctx, void* cuda_stream) {
     if (!ctx) { zk_set_error("set_stream: ctx is null"); return ZK_ERR_INVALID; }
     std::lock_guard<std::mutex> lk(ctx->mu);
-    ctx->stream = cuda_stream ? (cudaStream_t)cuda_stream : ctx->own_stream;
+    cudaStream_t next = cuda_stream ? (cudaStream_t)cuda_stream : ctx->own_stream;
+    if (next == ctx->stream) return ZK_OK;
+    // Several calls return with kernels still queued that read the context's scratch (the NTT's second buffer, the expression
+    // program, the MSM workspace, ...).  The new stream waits for everything queued on the old one so far, without blocking the host.
+    ZK_CUDA(cudaSetDevice(ctx->device));
+    if (!ctx->ev_switch) ZK_CUDA(cudaEventCreateWithFlags(&ctx->ev_switch, cudaEventDisableTiming));
+    ZK_CUDA(cudaEventRecord(ctx->ev_switch, ctx->stream));
+    ZK_CUDA(cudaStreamWaitEvent(next, ctx->ev_switch, 0));
+    ctx->stream = next;
+    ctx_update_pinned(ctx);
     return ZK_OK;
 }
 
@@ -344,6 +362,7 @@ int zk_ctx_set_profile(zk_ctx* ctx, int enabled) {
     std::lock_guard<std::mutex> lk(ctx->mu);
     ctx->ws.profile = enabled != 0;
     ctx->profile = enabled != 0;
+    ctx_update_pinned(ctx);
     return ZK_OK;
 }
 
@@ -359,6 +378,7 @@ int zk_ctx_set_option(zk_ctx* ctx, const char* name, long value) {
     if (!strcmp(name, "ctx_lanes")) {
         if (value < 1 || value > 16) { zk_set_error("set_option: ctx_lanes %ld outside [1, 16]", value); return ZK_ERR_INVALID; }
         ctx->n_lanes = (int)value;       // lanes already created stay allocated; fewer are used from now on
+        ctx_update_pinned(ctx);
         return ZK_OK;
     }
     if (!strcmp(name, "msm_batch")) {

@@ -1,6 +1,7 @@
 // ctx.hpp — the objects behind the opaque handles of include/zkb200.h, and the host-side helpers every entry point shares: the
 // field_id / curve_id dispatch, the argument checks and the context's scratch memory.
 #pragma once
+#include <atomic>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -113,6 +114,7 @@ struct zk_ctx {
     cudaStream_t side[SIDE_STREAMS] = {};
     int batch = (int)zkb::MSM_MAX_BATCH; // zk_ctx_set_option("msm_batch"): MSMs of one call fused into one pipeline
     cudaEvent_t ev_fork = nullptr;
+    cudaEvent_t ev_switch = nullptr;     // zk_ctx_set_stream: the new stream waits for the old one
     zkb::DevScratch d_scalars;           // staging for host-pointer MSM calls
     zkb::DevScratch d_ntt;               // staging for host-pointer NTT calls
     zkb::DevScratch d_ntt_tmp;           // second buffer of the two-pass plan
@@ -131,6 +133,7 @@ struct zk_ctx {
     zkb::DevScratch d_perm;              // zk_perm_aggreg_dev: den, then num / den over d1 | block products | final-value flag
     uint64_t launches = 0;
     bool profile = false;                // per-stage device timing (zk_ctx_set_profile)
+    std::atomic<bool> pinned{false};     // host-pointer calls stay on the primary lane (stream, profile, n_lanes; written under mu)
     cudaEvent_t ev_ntt[2] = {nullptr, nullptr};
     float ntt_ms = 0;                    // device time of the last profiled NTT call (all its kernels)
     // frees the scratch members; hidden like the library's other C++ symbols (zkb200.h gives the type default visibility)

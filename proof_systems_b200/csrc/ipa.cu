@@ -290,9 +290,9 @@ int zk_ipa_read(zk_ipa* s, uint64_t* out_a, uint64_t* out_b, size_t capacity, ui
     std::lock_guard<std::mutex> lk(ctx->mu);
     ZK_CUDA(cudaSetDevice(ctx->device));
     const size_t m = s->n < capacity ? s->n : capacity;
+    if (out_a && m) ZK_CUDA(cudaMemcpyAsync(out_a, s->d_a, m * sizeof(fe), cudaMemcpyDeviceToHost, ctx->stream));
+    if (out_b && m) ZK_CUDA(cudaMemcpyAsync(out_b, s->d_b, m * sizeof(fe), cudaMemcpyDeviceToHost, ctx->stream));
     ZK_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (out_a && m) ZK_CUDA(cudaMemcpy(out_a, s->d_a, m * sizeof(fe), cudaMemcpyDeviceToHost));
-    if (out_b && m) ZK_CUDA(cudaMemcpy(out_b, s->d_b, m * sizeof(fe), cudaMemcpyDeviceToHost));
     if (out_g_xyz) {
         if (s->n != 1) { zk_set_error("ipa_read: the folded base is available after the last round only"); return ZK_ERR_INVALID; }
         const size_t len = s->n0 < s->bases->b.n ? s->n0 : s->bases->b.n;

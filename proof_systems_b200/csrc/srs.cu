@@ -117,7 +117,8 @@ int zk_srs_get_lagrange_basis(zk_srs* srs, size_t domain_size, uint64_t* out_xy,
     if (capacity_points < total) { zk_set_error("get_lagrange_basis: capacity %zu < %zu", capacity_points, total); return ZK_ERR_INVALID; }
     std::lock_guard<std::mutex> lk(srs->ctx->mu);
     ZK_CUDA(cudaSetDevice(srs->ctx->device));
-    ZK_CUDA(cudaMemcpy(out_xy, it->second->b.d_points, total * sizeof(affine_t), cudaMemcpyDeviceToHost));
+    ZK_CUDA(cudaMemcpyAsync(out_xy, it->second->b.d_points, total * sizeof(affine_t), cudaMemcpyDeviceToHost, srs->ctx->stream));
+    ZK_CUDA(cudaStreamSynchronize(srs->ctx->stream));
     return ZK_OK;
 }
 
