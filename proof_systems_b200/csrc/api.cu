@@ -62,22 +62,22 @@ int ctx_msm_many_offs(zk_ctx* ctx, const zk_bases* bases, const size_t* offs, si
     // MSMs per pipeline: the context's limit, and no more than keeps the sorted entry list below 2^28 entries (1 GiB of scratch)
     const unsigned c_eff = bases->b.c ? bases->b.c : (window_bits ? (unsigned)window_bits : (unsigned)msm_default_window(n, false));
     const size_t per_msm = std::max<size_t>(1, (n + n_extra) * msm_num_windows(std::max(2u, c_eff)));
-    size_t fuse = std::min<size_t>((size_t)std::max(1, ctx->batch), std::max<size_t>(1, ((size_t)1 << 28) / per_msm));
+    size_t fuse = std::min<size_t>((size_t)std::max(1, ctx->msm.batch), std::max<size_t>(1, ((size_t)1 << 28) / per_msm));
     if (ctx->profile) fuse = 1;   // stage times are those of ONE MSM (zk_ctx_last_stage_ms)
     for (size_t j0 = 0; j0 < k; j0 += fuse) {
         const unsigned cnt = (unsigned)std::min(fuse, k - j0);
         MsmResultShape shape;
         unsigned nl = 0;
-        ctx->ws.h_slot = 0;
         const int rc = with_curve(bases->b.curve, [&](auto c) {
             using C = decltype(c);
-            if (int e = msm_run<typename C::F, typename C::FS>(bases->b, offs + j0, n, d_scalars + j0, cnt, mont != 0, (unsigned)window_bits, ctx->ws,
-                                                               ctx->stream, &shape, &nl, d_extra, n_extra))
+            if (int e = msm_run<typename C::F, typename C::FS>(bases->b, offs + j0, n, d_scalars + j0, cnt, mont != 0, (unsigned)window_bits, d_extra,
+                                                               n_extra, ctx->msm, ctx->sm_count, ctx->profile, ctx->ws, ctx->stream, nullptr, 0,
+                                                               &shape, &nl))
                 return e;
             ctx->launches += nl;
             for (unsigned j = 0; j < cnt; j++) {
                 host::hxyzz r = host::identity();
-                if (shape.groups) r = msm_finish_t<typename C::HP>(ctx->ws.h_bitsums + (size_t)j * shape.groups * shape.c, shape.c, shape.groups);
+                if (shape.groups) r = msm_finish_t<typename C::HP>(ctx->ws.h_bitsums.at<xyzz_t>() + (size_t)j * shape.groups * shape.c, shape.c, shape.groups);
                 xyzz_to_jac_out(bases->b.curve, r, out_xyz + 12 * (j0 + j));
             }
             return ZK_OK;
@@ -90,6 +90,70 @@ int ctx_msm_many_offs(zk_ctx* ctx, const zk_bases* bases, const size_t* offs, si
 int ctx_msm_device(zk_ctx* ctx, const zk_bases* bases, size_t off, size_t n, const fe* d_scalars, int mont, int window_bits,
                    uint64_t out_xyz[12]) {
     return ctx_msm_many(ctx, bases, off, n, &d_scalars, 1, mont, window_bits, out_xyz);
+}
+
+// The `count` scalars of a call where the recode kernel reads them.  Page-locked host memory (cudaHostAlloc / cudaHostRegister) is
+// read in place over PCIe (unified addressing): no staging copy, the transfer is fused into the first kernel.  Device or managed
+// memory is read in place when `device_ok`.  Anything else is staged in ctx->d_scalars.
+static int msm_scalars_on_device(zk_ctx* ctx, const void* scalars, size_t count, bool device_ok, const fe** out) {
+    cudaPointerAttributes attr;
+    const bool known = cudaPointerGetAttributes(&attr, scalars) == cudaSuccess;
+    if (!known) cudaGetLastError();   // clear the "invalid value" some drivers report for pageable pointers
+    if (known && attr.type == cudaMemoryTypeHost && attr.devicePointer) {
+        *out = (const fe*)attr.devicePointer;
+    } else if (known && device_ok && (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged)) {
+        *out = (const fe*)scalars;
+    } else {
+        if (int rc = ctx->d_scalars.ensure(std::max<size_t>(count, 1) * sizeof(fe))) return rc;
+        *out = ctx->d_scalars.at<fe>();
+        if (count) ZK_CUDA(cudaMemcpyAsync(ctx->d_scalars.p, scalars, count * sizeof(fe), cudaMemcpyHostToDevice, ctx->stream));
+    }
+    return ZK_OK;
+}
+
+// Multi-GPU sharding (SURVEY.md §8e): this rank's MSM is left on the device as its slice sums and nothing is synchronised, so
+// the caller can enqueue the all-gather on the same stream while the kernels still run.
+int ctx_msm_partial(zk_ctx* ctx, const zk_bases* bases, size_t off, size_t n, const void* scalars, int scalars_are_mont, int window_bits,
+                    void* d_out, size_t capacity_points, unsigned* out_c, unsigned* out_groups) {
+    if (!ctx || !bases || !d_out || !out_c || !out_groups || (!scalars && n)) { zk_set_error("msm_partial: null argument"); return ZK_ERR_INVALID; }
+    if (ctx_root(bases->ctx) != ctx_root(ctx)) { zk_set_error("msm: bases belong to another context"); return ZK_ERR_INVALID; }
+    if (window_bits < 0 || window_bits > (int)MSM_MAX_WINDOW_BITS) { zk_set_error("msm: window_bits %d outside [0, %u]", window_bits, MSM_MAX_WINDOW_BITS); return ZK_ERR_INVALID; }
+    if (n == 0) { zk_set_error("msm_partial: empty slice"); return ZK_ERR_INVALID; }
+    const fe* d_sc = nullptr;
+    if (int rc = msm_scalars_on_device(ctx, scalars, n, true, &d_sc)) return rc;
+    MsmResultShape shape;
+    unsigned nl = 0;
+    int rc = with_curve(bases->b.curve, [&](auto c) {
+        using C = decltype(c);
+        return msm_run<typename C::F, typename C::FS>(bases->b, &off, n, &d_sc, 1, scalars_are_mont != 0, (unsigned)window_bits, nullptr, 0, ctx->msm,
+                                                      ctx->sm_count, ctx->profile, ctx->ws, ctx->stream, (xyzz_t*)d_out, capacity_points, &shape, &nl);
+    });
+    ctx->launches += nl;
+    if (rc) return rc;
+    *out_c = shape.c;
+    *out_groups = shape.groups;
+    return ZK_OK;
+}
+
+// d_all: `world` gathered partials of zk_msm_partial (device, world x groups*c points, same shape on every rank).  Sums them
+// per slice on the device, copies groups*c points to the host and finishes the O(c) tail there.
+int ctx_msm_finish_gathered(zk_ctx* ctx, int curve_id, const void* d_all, size_t world, unsigned c, unsigned groups, uint64_t out_xyz[12]) {
+    if (!ctx || !d_all || !out_xyz || world == 0) { zk_set_error("msm_finish_gathered: null argument"); return ZK_ERR_INVALID; }
+    if (int rc = check_curve("msm_finish_gathered", curve_id)) return rc;
+    const size_t count = (size_t)c * groups;
+    if (count == 0 || count > 4096) { zk_set_error("msm_finish_gathered: bad shape c = %u, groups = %u", c, groups); return ZK_ERR_INVALID; }
+    if (int rc = ctx->d_gather_sum.ensure(count * sizeof(xyzz_t))) return rc;
+    if (int rc = ctx->h_gather.ensure(count * sizeof(xyzz_t))) return rc;
+    xyzz_t *d_sum = ctx->d_gather_sum.at<xyzz_t>(), *h_sum = ctx->h_gather.at<xyzz_t>();
+    return with_curve(curve_id, [&](auto cv) {
+        using C = decltype(cv);
+        if (int e = msm_sum_partials<typename C::F>((const xyzz_t*)d_all, world, count, d_sum, ctx->stream)) return e;
+        ctx->launches += 1;
+        ZK_CUDA(cudaMemcpyAsync(h_sum, d_sum, count * sizeof(xyzz_t), cudaMemcpyDeviceToHost, ctx->stream));
+        ZK_CUDA(cudaStreamSynchronize(ctx->stream));
+        xyzz_to_jac_out(curve_id, msm_finish_t<typename C::HP>(h_sum, c, groups), out_xyz);
+        return ZK_OK;
+    });
 }
 
 static int ctx_side_streams_init(zk_ctx* ctx) {
@@ -182,7 +246,7 @@ static int ctx_init_lane(zk_ctx* c, int device_id) {
     if (se != cudaSuccess) { zk_set_error("cudaStreamCreate: %s", cudaGetErrorString(se)); return ZK_ERR_CUDA; }
     c->stream = c->own_stream;
     cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device_id) == cudaSuccess) c->ws.sm_count = prop.multiProcessorCount;
+    if (cudaGetDeviceProperties(&prop, device_id) == cudaSuccess) c->sm_count = prop.multiProcessorCount;
     return ZK_OK;
 }
 
@@ -210,7 +274,7 @@ int ctx_acquire_lane(zk_ctx* ctx, LaneLock& out) {
             zk_ctx* c = new zk_ctx();
             c->parent = ctx;
             if (cudaSetDevice(ctx->device) != cudaSuccess || ctx_init_lane(c, ctx->device) != ZK_OK) { delete c; break; }
-            c->batch = ctx->batch; c->ws.chunk = ctx->ws.chunk; c->ws.wave_threads = ctx->ws.wave_threads; c->ws.tma_gather = ctx->ws.tma_gather;
+            c->msm = ctx->msm;
             ctx->children.push_back(c);
         }
         lanes.push_back(ctx);
@@ -322,7 +386,6 @@ void zk_ctx_destroy(zk_ctx* ctx) {
     ctx->children.clear();
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
-    msm_workspace_free(ctx->ws);
     for (int l = 0; l < zk_ctx::SIDE_STREAMS; l++)
         if (ctx->side[l]) { cudaStreamSynchronize(ctx->side[l]); cudaStreamDestroy(ctx->side[l]); }
     if (ctx->ev_fork) cudaEventDestroy(ctx->ev_fork);
@@ -360,7 +423,6 @@ uint64_t zk_ctx_launch_count(const zk_ctx* ctx) {
 int zk_ctx_set_profile(zk_ctx* ctx, int enabled) {
     if (!ctx) { zk_set_error("set_profile: ctx is null"); return ZK_ERR_INVALID; }
     std::lock_guard<std::mutex> lk(ctx->mu);
-    ctx->ws.profile = enabled != 0;
     ctx->profile = enabled != 0;
     ctx_update_pinned(ctx);
     return ZK_OK;
@@ -369,38 +431,27 @@ int zk_ctx_set_profile(zk_ctx* ctx, int enabled) {
 int zk_ctx_set_option(zk_ctx* ctx, const char* name, long value) {
     if (!ctx || !name) { zk_set_error("set_option: null argument"); return ZK_ERR_INVALID; }
     std::lock_guard<std::mutex> lk(ctx->mu);
-    if (!strcmp(name, "msm_chunk")) {
-        if (value < 0 || value > 4096) { zk_set_error("set_option: msm_chunk %ld outside [0, 4096]", value); return ZK_ERR_INVALID; }
-        ctx->ws.chunk = (uint32_t)value;
-        for (zk_ctx* c : ctx->children) c->ws.chunk = (uint32_t)value;
-        return ZK_OK;
-    }
     if (!strcmp(name, "ctx_lanes")) {
         if (value < 1 || value > 16) { zk_set_error("set_option: ctx_lanes %ld outside [1, 16]", value); return ZK_ERR_INVALID; }
         ctx->n_lanes = (int)value;       // lanes already created stay allocated; fewer are used from now on
         ctx_update_pinned(ctx);
         return ZK_OK;
     }
-    if (!strcmp(name, "msm_batch")) {
+    if (!strcmp(name, "msm_chunk")) {
+        if (value < 0 || value > 4096) { zk_set_error("set_option: msm_chunk %ld outside [0, 4096]", value); return ZK_ERR_INVALID; }
+        ctx->msm.chunk = (uint32_t)value;
+    } else if (!strcmp(name, "msm_batch")) {
         if (value < 1 || value > (long)MSM_MAX_BATCH) { zk_set_error("set_option: msm_batch %ld outside [1, %u]", value, MSM_MAX_BATCH); return ZK_ERR_INVALID; }
-        ctx->batch = (int)value;
-        for (zk_ctx* c : ctx->children) c->batch = (int)value;
-        return ZK_OK;
-    }
-    if (!strcmp(name, "msm_tma")) {
-        if (value < 0 || value > 1) { zk_set_error("set_option: msm_tma %ld outside [0, 1]", value); return ZK_ERR_INVALID; }
-        ctx->ws.tma_gather = value != 0;
-        for (zk_ctx* c : ctx->children) c->ws.tma_gather = value != 0;
-        return ZK_OK;
-    }
-    if (!strcmp(name, "msm_wave_threads")) {
+        ctx->msm.batch = (int)value;
+    } else if (!strcmp(name, "msm_wave_threads")) {
         if (value < 0 || value > 2048) { zk_set_error("set_option: msm_wave_threads %ld outside [0, 2048]", value); return ZK_ERR_INVALID; }
-        ctx->ws.wave_threads = (uint32_t)value;
-        for (zk_ctx* c : ctx->children) c->ws.wave_threads = (uint32_t)value;
-        return ZK_OK;
+        ctx->msm.wave_threads = (uint32_t)value;
+    } else {
+        zk_set_error("set_option: unknown option '%s'", name);
+        return ZK_ERR_INVALID;
     }
-    zk_set_error("set_option: unknown option '%s'", name);
-    return ZK_ERR_INVALID;
+    for (zk_ctx* c : ctx->children) c->msm = ctx->msm;
+    return ZK_OK;
 }
 
 int zk_ctx_last_stage_ms(const zk_ctx* ctx, float* out, size_t capacity) {
@@ -518,82 +569,11 @@ int zk_msm_batch(zk_ctx* root, const zk_bases* bases, size_t off, size_t n, cons
     zk_ctx* ctx = ll.lane;
     ZK_CUDA(cudaSetDevice(ctx->device));
     if (k == 0) return ZK_OK;
-    // Scalars in page-locked (cudaHostAlloc / cudaHostRegister) memory are read by the recode kernel straight over PCIe
-    // (unified addressing): no staging copy, the transfer is fused into the first kernel.  Pageable memory is staged.
     const fe* d_sc = nullptr;
-    int rc = ZK_OK;
-    cudaPointerAttributes attr;
-    if (n && cudaPointerGetAttributes(&attr, scalars) == cudaSuccess && attr.type == cudaMemoryTypeHost && attr.devicePointer) {
-        d_sc = (const fe*)attr.devicePointer;
-    } else {
-        cudaGetLastError();  // clear the "invalid value" some drivers report for pageable pointers
-        rc = ctx->d_scalars.ensure(std::max<size_t>(k * n, 1) * sizeof(fe));
-        if (rc) return rc;
-        d_sc = ctx->d_scalars.at<fe>();
-        if (n) ZK_CUDA(cudaMemcpyAsync(ctx->d_scalars.p, scalars, k * n * sizeof(fe), cudaMemcpyHostToDevice, ctx->stream));
-    }
+    if (int rc = msm_scalars_on_device(ctx, scalars, k * n, false, &d_sc)) return rc;
     std::vector<const fe*> scs(k);
     for (size_t j = 0; j < k; j++) scs[j] = d_sc + j * n;
     return ctx_msm_many(ctx, bases, off, n, scs.data(), k, scalars_are_mont, window_bits, out_xyz);
-}
-
-// Multi-GPU sharding (SURVEY.md §8e): this rank's MSM is left on the device as its slice sums and nothing is synchronised, so
-// the caller can enqueue the all-gather on the same stream while the kernels still run.
-static int msm_partial_impl(zk_ctx* ctx, const zk_bases* bases, size_t off, size_t n, const void* scalars, int scalars_are_mont, int window_bits,
-                   void* d_out, size_t capacity_points, unsigned* out_c, unsigned* out_groups) {
-    if (!ctx || !bases || !d_out || !out_c || !out_groups || (!scalars && n)) { zk_set_error("msm_partial: null argument"); return ZK_ERR_INVALID; }
-    if (ctx_root(bases->ctx) != ctx_root(ctx)) { zk_set_error("msm: bases belong to another context"); return ZK_ERR_INVALID; }
-    if (window_bits < 0 || window_bits > (int)MSM_MAX_WINDOW_BITS) { zk_set_error("msm: window_bits %d outside [0, %u]", window_bits, MSM_MAX_WINDOW_BITS); return ZK_ERR_INVALID; }
-    if (n == 0) { zk_set_error("msm_partial: empty slice"); return ZK_ERR_INVALID; }
-    const fe* d_sc = nullptr;
-    cudaPointerAttributes attr;
-    const bool known = cudaPointerGetAttributes(&attr, scalars) == cudaSuccess;
-    if (!known) cudaGetLastError();   // some drivers report "invalid value" for pageable pointers
-    if (known && (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged)) {
-        d_sc = (const fe*)scalars;
-    } else if (known && attr.type == cudaMemoryTypeHost && attr.devicePointer) {
-        d_sc = (const fe*)attr.devicePointer;          // page-locked: read over PCIe by the recode kernel
-    } else {
-        if (int rc = ctx->d_scalars.ensure(n * sizeof(fe))) return rc;
-        d_sc = ctx->d_scalars.at<fe>();
-        ZK_CUDA(cudaMemcpyAsync(ctx->d_scalars.p, scalars, n * sizeof(fe), cudaMemcpyHostToDevice, ctx->stream));
-    }
-    MsmResultShape shape;
-    unsigned nl = 0;
-    ctx->ws.d_T_out = (xyzz_t*)d_out;
-    ctx->ws.d_T_cap = capacity_points;
-    int rc = with_curve(bases->b.curve, [&](auto c) {
-        using C = decltype(c);
-        return msm_run<typename C::F, typename C::FS>(bases->b, &off, n, &d_sc, 1, scalars_are_mont != 0, (unsigned)window_bits, ctx->ws, ctx->stream, &shape, &nl);
-    });
-    ctx->ws.d_T_out = nullptr;
-    ctx->ws.d_T_cap = 0;
-    ctx->launches += nl;
-    if (rc) return rc;
-    *out_c = shape.c;
-    *out_groups = shape.groups;
-    return ZK_OK;
-}
-
-// d_all: `world` gathered partials of zk_msm_partial (device, world x groups*c points, same shape on every rank).  Sums them
-// per slice on the device, copies groups*c points to the host and finishes the O(c) tail there.
-static int msm_finish_gathered_impl(zk_ctx* ctx, int curve_id, const void* d_all, size_t world, unsigned c, unsigned groups, uint64_t out_xyz[12]) {
-    if (!ctx || !d_all || !out_xyz || world == 0) { zk_set_error("msm_finish_gathered: null argument"); return ZK_ERR_INVALID; }
-    if (int rc = check_curve("msm_finish_gathered", curve_id)) return rc;
-    const size_t count = (size_t)c * groups;
-    if (count == 0 || count > 4096) { zk_set_error("msm_finish_gathered: bad shape c = %u, groups = %u", c, groups); return ZK_ERR_INVALID; }
-    if (int rc = ctx->d_gather_sum.ensure(count * sizeof(xyzz_t))) return rc;
-    if (int rc = ctx->h_gather.ensure(count * sizeof(xyzz_t))) return rc;
-    xyzz_t *d_sum = ctx->d_gather_sum.at<xyzz_t>(), *h_sum = ctx->h_gather.at<xyzz_t>();
-    return with_curve(curve_id, [&](auto cv) {
-        using C = decltype(cv);
-        if (int e = msm_sum_partials<typename C::F>((const xyzz_t*)d_all, world, count, d_sum, ctx->stream)) return e;
-        ctx->launches += 1;
-        ZK_CUDA(cudaMemcpyAsync(h_sum, d_sum, count * sizeof(xyzz_t), cudaMemcpyDeviceToHost, ctx->stream));
-        ZK_CUDA(cudaStreamSynchronize(ctx->stream));
-        xyzz_to_jac_out(curve_id, msm_finish_t<typename C::HP>(h_sum, c, groups), out_xyz);
-        return ZK_OK;
-    });
 }
 
 int zk_msm_partial(zk_ctx* ctx, const zk_bases* bases, size_t off, size_t n, const void* scalars, int scalars_are_mont, int window_bits,
@@ -601,13 +581,13 @@ int zk_msm_partial(zk_ctx* ctx, const zk_bases* bases, size_t off, size_t n, con
     if (!ctx) { zk_set_error("msm_partial: null argument"); return ZK_ERR_INVALID; }
     std::lock_guard<std::mutex> lk(ctx->mu);
     ZK_CUDA(cudaSetDevice(ctx->device));
-    return msm_partial_impl(ctx, bases, off, n, scalars, scalars_are_mont, window_bits, d_out, capacity_points, out_c, out_groups);
+    return ctx_msm_partial(ctx, bases, off, n, scalars, scalars_are_mont, window_bits, d_out, capacity_points, out_c, out_groups);
 }
 int zk_msm_finish_gathered(zk_ctx* ctx, int curve_id, const void* d_all, size_t world, unsigned c, unsigned groups, uint64_t out_xyz[12]) {
     if (!ctx) { zk_set_error("msm_finish_gathered: null argument"); return ZK_ERR_INVALID; }
     std::lock_guard<std::mutex> lk(ctx->mu);
     ZK_CUDA(cudaSetDevice(ctx->device));
-    return msm_finish_gathered_impl(ctx, curve_id, d_all, world, c, groups, out_xyz);
+    return ctx_msm_finish_gathered(ctx, curve_id, d_all, world, c, groups, out_xyz);
 }
 
 int zk_msm(zk_ctx* ctx, const zk_bases* bases, size_t off, size_t n, const uint64_t* scalars, int scalars_are_mont, int window_bits, uint64_t out_xyz[12]) {
@@ -802,7 +782,7 @@ int zk_debug_op_throughput(zk_ctx* ctx, int field_id, int kind, unsigned blocks,
     DevScratch dout;                     // transient, like the events: freed on every return
     if (int rc = dout.ensure(sizeof(xyzz_t))) return rc;
     xyzz_t* d = dout.at<xyzz_t>();
-    struct Event { cudaEvent_t e = nullptr; ~Event() { if (e) cudaEventDestroy(e); } } e0, e1;
+    Event e0, e1;
     ZK_CUDA(cudaEventCreate(&e0.e));
     ZK_CUDA(cudaEventCreate(&e1.e));
     for (int rep = 0; rep < 2; rep++) {  // first launch warms up
@@ -833,13 +813,3 @@ int zk_debug_mul_throughput(zk_ctx* ctx, int field_id, unsigned iters, double* o
 }
 
 }  // extern "C"
-
-namespace zkb {
-int ctx_msm_partial_nolock(zk_ctx* ctx, const zk_bases* bases, size_t off, size_t n, const void* scalars, int scalars_are_mont, int window_bits,
-                           void* d_out, size_t capacity_points, unsigned* out_c, unsigned* out_groups) {
-    return msm_partial_impl(ctx, bases, off, n, scalars, scalars_are_mont, window_bits, d_out, capacity_points, out_c, out_groups);
-}
-int ctx_msm_finish_gathered_nolock(zk_ctx* ctx, int curve_id, const void* d_all, size_t world, unsigned c, unsigned groups, uint64_t out_xyz[12]) {
-    return msm_finish_gathered_impl(ctx, curve_id, d_all, world, c, groups, out_xyz);
-}
-}  // namespace zkb

@@ -71,12 +71,6 @@ struct zk_comm {
     size_t cap_points = 0;
 };
 
-namespace zkb {
-int ctx_msm_partial_nolock(zk_ctx* ctx, const zk_bases* bases, size_t off, size_t n, const void* scalars, int scalars_are_mont, int window_bits,
-                           void* d_out, size_t capacity_points, unsigned* out_c, unsigned* out_groups);                       // api.cu
-int ctx_msm_finish_gathered_nolock(zk_ctx* ctx, int curve_id, const void* d_all, size_t world, unsigned c, unsigned groups, uint64_t out_xyz[12]);
-}
-
 extern "C" {
 
 int zk_comm_unique_id(uint8_t out_id[128]) {
@@ -136,14 +130,14 @@ int zk_msm_sharded(zk_comm* c, const zk_bases* bases, size_t off, size_t n, cons
         c->cap_points = MAX_POINTS;
     }
     unsigned cc = 0, groups = 0;
-    int rc = ctx_msm_partial_nolock(ctx, bases, off, n, scalars, scalars_are_mont, window_bits, c->d_mine, c->cap_points, &cc, &groups);
+    int rc = ctx_msm_partial(ctx, bases, off, n, scalars, scalars_are_mont, window_bits, c->d_mine, c->cap_points, &cc, &groups);
     if (rc) return rc;
     const size_t cnt = (size_t)cc * groups;
-    if (c->world == 1) return ctx_msm_finish_gathered_nolock(ctx, bases->b.curve, c->d_mine, 1, cc, groups, out_xyz);
+    if (c->world == 1) return ctx_msm_finish_gathered(ctx, bases->b.curve, c->d_mine, 1, cc, groups, out_xyz);
     // the collective rides the context's stream behind the kernels: no host synchronisation between the MSM and the exchange
     rc = nccl_check(nccl().AllGather(c->d_mine, c->d_all, cnt * sizeof(xyzz_t), NCCL_UINT8, c->comm, ctx->stream), "ncclAllGather");
     if (rc) return rc;
-    return ctx_msm_finish_gathered_nolock(ctx, bases->b.curve, c->d_all, (size_t)c->world, cc, groups, out_xyz);
+    return ctx_msm_finish_gathered(ctx, bases->b.curve, c->d_all, (size_t)c->world, cc, groups, out_xyz);
 }
 
 }  // extern "C"

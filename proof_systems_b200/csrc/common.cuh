@@ -1,4 +1,4 @@
-// common.cuh — error handling, vectorised element access, library-wide ids.
+// common.cuh — error handling, self-freeing scratch memory and events, vectorised element access, library-wide ids.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -21,6 +21,46 @@ void zk_set_error(const char* fmt, ...);
             return ZK_ERR_CUDA;                                                       \
         }                                                                                  \
     } while (0)
+
+// Memory that grows on demand (the contents are not kept) and is freed with its owner: device memory, or page-locked host memory
+// with PINNED.  zk_ctx_destroy makes the context's device current before its members are destroyed.
+template <bool PINNED> struct Scratch {
+    void* p = nullptr;
+    size_t cap = 0;
+    Scratch() = default;
+    Scratch(const Scratch&) = delete;
+    Scratch& operator=(const Scratch&) = delete;
+    ~Scratch() { release(); }
+    void release() {
+        if (p) PINNED ? cudaFreeHost(p) : cudaFree(p);
+        p = nullptr, cap = 0;
+    }
+    int ensure(size_t bytes) {
+        if (cap >= bytes) return ZK_OK;
+        release();
+        ZK_CUDA(PINNED ? cudaMallocHost(&p, bytes) : cudaMalloc(&p, bytes));
+        cap = bytes;
+        return ZK_OK;
+    }
+    template <class T> T* at(size_t byte_off = 0) const { return (T*)((char*)p + byte_off); }
+};
+using DevScratch = Scratch<false>;
+using PinnedScratch = Scratch<true>;
+
+// sub-buffers of one scratch allocation: add() hands out 256-byte aligned offsets in order, total is the size to ensure
+struct Layout {
+    size_t total = 0;
+    size_t add(size_t bytes) { const size_t off = (total + 255) & ~(size_t)255; total = off + bytes; return off; }
+};
+
+// a CUDA event destroyed with its owner
+struct Event {
+    cudaEvent_t e = nullptr;
+    Event() = default;
+    Event(const Event&) = delete;
+    Event& operator=(const Event&) = delete;
+    ~Event() { if (e) cudaEventDestroy(e); }
+};
 
 // 128-bit vector access: an fe is two uint4, an affine point four, an XYZZ point eight.
 __device__ __forceinline__ fe load_fe(const fe* p) {

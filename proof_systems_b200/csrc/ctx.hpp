@@ -50,37 +50,6 @@ inline bool canonical(int field_id, const uint64_t* x) {
     return with_field(field_id, [&](auto f) { return !host::geq_mod<typename decltype(f)::Host>(x); });
 }
 
-// Memory that grows on demand (the contents are not kept) and is freed with its owner: device memory, or page-locked host memory
-// with PINNED.  zk_ctx_destroy makes the context's device current before its members are destroyed.
-template <bool PINNED> struct Scratch {
-    void* p = nullptr;
-    size_t cap = 0;
-    Scratch() = default;
-    Scratch(const Scratch&) = delete;
-    Scratch& operator=(const Scratch&) = delete;
-    ~Scratch() { release(); }
-    void release() {
-        if (p) PINNED ? cudaFreeHost(p) : cudaFree(p);
-        p = nullptr, cap = 0;
-    }
-    int ensure(size_t bytes) {
-        if (cap >= bytes) return ZK_OK;
-        release();
-        ZK_CUDA(PINNED ? cudaMallocHost(&p, bytes) : cudaMalloc(&p, bytes));
-        cap = bytes;
-        return ZK_OK;
-    }
-    template <class T> T* at(size_t byte_off = 0) const { return (T*)((char*)p + byte_off); }
-};
-using DevScratch = Scratch<false>;
-using PinnedScratch = Scratch<true>;
-
-// sub-buffers of one scratch allocation: add() hands out 256-byte aligned offsets in order, total is the size to ensure
-struct Layout {
-    size_t total = 0;
-    size_t add(size_t bytes) { const size_t off = (total + 255) & ~(size_t)255; total = off + bytes; return off; }
-};
-
 // a context's pinned slots for small read-backs (ctx_pinned), one per use
 struct PinnedSlots {
     fe ip[2];                   // the IPA rounds' two inner products; zk_srs_open: the combined inner product, then a0
@@ -107,12 +76,13 @@ struct zk_ctx {
     std::mutex pool_mu;                        // children list
     std::mutex tab_mu;                         // NTT table cache of the primary lane (shared by all lanes)
     int device = 0;
+    int sm_count = 132;                        // SMs of the device (the MSM sizes its grids by them)
     cudaStream_t own_stream = nullptr, stream = nullptr;
     std::mutex mu;                       // a context serialises its calls (SRS: Sync + Send, SURVEY.md §8b "Threading")
     zkb::MsmWorkspace ws;                // scratch of the MSM pipeline (runs on `stream`)
     static constexpr int SIDE_STREAMS = 2;   // copy-in / copy-out streams of the pipelined host-pointer NTT (zk_ntt_batch)
     cudaStream_t side[SIDE_STREAMS] = {};
-    int batch = (int)zkb::MSM_MAX_BATCH; // zk_ctx_set_option("msm_batch"): MSMs of one call fused into one pipeline
+    zkb::MsmTuning msm;                  // zk_ctx_set_option("msm_batch", "msm_chunk", "msm_wave_threads")
     cudaEvent_t ev_fork = nullptr;
     cudaEvent_t ev_switch = nullptr;     // zk_ctx_set_stream: the new stream waits for the old one
     zkb::DevScratch d_scalars;           // staging for host-pointer MSM calls
@@ -122,7 +92,7 @@ struct zk_ctx {
     std::map<unsigned, zkb::NttTables> ntt_tables;                         // key: field | inverse << 1 | log_n << 2
     zkb::DevScratch d_gather_sum;        // zk_msm_finish_gathered: cross-rank sums of the slice sums
     zkb::PinnedScratch h_gather;         // ... and their pinned host copy
-    zkb::PinnedScratch h_slots;          // zkb::PinnedSlots, through ctx_pinned
+    zkb::PinnedScratch h_pinned_slots;   // zkb::PinnedSlots, through ctx_pinned
     zkb::DevScratch d_open;              // zk_srs_open: staged polynomials | evaluation part | descriptors | extra bases
     zkb::DevScratch d_flag;              // zk_poly_divide_by_vanishing_dev: remainder flag
     zkb::DevScratch d_expr;              // zk_expr_eval_dev: program | constants | column table
@@ -157,20 +127,24 @@ inline const zk_ctx* ctx_root(const zk_ctx* c) { return c && c->parent ? c->pare
 int ctx_msm_device(zk_ctx* ctx, const zk_bases* bases, size_t off, size_t n, const fe* d_scalars, int mont, int window_bits,
                    uint64_t out_xyz[12]);
 // the context's pinned slots, allocated on first use; null (the error set) when that fails
-inline PinnedSlots* ctx_pinned(zk_ctx* ctx) { return ctx->h_slots.ensure(sizeof(PinnedSlots)) ? nullptr : ctx->h_slots.at<PinnedSlots>(); }
+inline PinnedSlots* ctx_pinned(zk_ctx* ctx) { return ctx->h_pinned_slots.ensure(sizeof(PinnedSlots)) ? nullptr : ctx->h_pinned_slots.at<PinnedSlots>(); }
 // the unscaled twiddle tables of a forward / inverse transform (pointwise evaluators take x_i = w^i from them)
 int ctx_ntt_table_ptrs(zk_ctx* ctx, int field, unsigned log_n, bool inverse, const fe** ulo, const fe** mid, const fe** hi2);
 // the NTT of zk_ntt_dev without the context lock (the caller holds it)
 int ctx_ntt_device(zk_ctx* ctx, int field, fe* d_data, unsigned log_n, size_t batch, size_t in_len, int inverse, int coset);
 int ctx_ntt_device_oop(zk_ctx* ctx, int field, const fe* d_in, size_t in_bs, fe* d_out, unsigned log_n, size_t batch, size_t in_len, int inverse, int coset);
 // k independent MSMs over the same bases slice [off, off + n), scalars j at d_scalars[j] (device memory, ordered after
-// ctx->stream), fused into pipelines of up to ctx->batch MSMs (msm.cuh).  Results (Jacobian) to out_xyz + 12 j.
+// ctx->stream), fused into pipelines of up to ctx->msm.batch MSMs (msm.cuh).  Results (Jacobian) to out_xyz + 12 j.
 // d_extra / n_extra: points of this call only, laid out like the table (msm.cuh); every scalar vector then has n + n_extra entries.
 int ctx_msm_many(zk_ctx* ctx, const zk_bases* bases, size_t off, size_t n, const fe* const* d_scalars, size_t k, int mont, int window_bits,
                  uint64_t* out_xyz, const affine_t* d_extra = nullptr, size_t n_extra = 0);
 // the same with one base offset per MSM (the chunks of a chunked Lagrange basis share their scalars, not their bases)
 int ctx_msm_many_offs(zk_ctx* ctx, const zk_bases* bases, const size_t* offs, size_t n, const fe* const* d_scalars, size_t k, int mont, int window_bits,
                       uint64_t* out_xyz, const affine_t* d_extra = nullptr, size_t n_extra = 0);
+// zk_msm_partial / zk_msm_finish_gathered without the context lock (the caller holds it)
+int ctx_msm_partial(zk_ctx* ctx, const zk_bases* bases, size_t off, size_t n, const void* scalars, int scalars_are_mont, int window_bits,
+                    void* d_out, size_t capacity_points, unsigned* out_c, unsigned* out_groups);
+int ctx_msm_finish_gathered(zk_ctx* ctx, int curve_id, const void* d_all, size_t world, unsigned c, unsigned groups, uint64_t out_xyz[12]);
 }  // namespace zkb
 
 // host-side mirror of poly_commitment::ipa::SRS<G> (srs.cu); shared with the opening proof (open.cu)

@@ -275,89 +275,6 @@ __global__ void __launch_bounds__(128) k_accumulate(const affine_t* __restrict__
     store_xyzz(sb == 1 ? buckets + b : partials + t, acc);
 }
 
-// ---------------------------------------------------------------------------------------------- accumulation, TMA-staged gather
-// The same accumulation with the gather moved to the bulk asynchronous copy engine (TMA, `cp.async.bulk`; UBLKCP in SASS): every lane
-// asks the copy engine for its next 64-byte point, to be dropped in its own shared-memory slot and signalled on the warp's mbarrier,
-// while it adds the current one — two stages per lane.  BASELINE's north star names this staging; whether it pays is measured, not
-// assumed (zk_ctx_set_option "msm_tma", tools/msm_tma_ab.py): the kernel is bound by the integer multiply-add pipe, not by its loads,
-// so taking the loads off the LSU path buys nothing and the shared-memory round trip costs a little.
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t mbar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(mbar), "r"(count) : "memory"); }
-__device__ __forceinline__ void mbar_arrive(uint32_t mbar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(mbar) : "memory"); }
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t mbar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mbar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t mbar, uint32_t parity) {
-    uint32_t done;
-    do {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(done) : "r"(mbar), "r"(parity) : "memory");
-    } while (!done);
-}
-__device__ __forceinline__ void bulk_copy_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t mbar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(mbar) : "memory");
-}
-
-template <class F>
-__global__ void __launch_bounds__(128) k_accumulate_tma(const affine_t* __restrict__ points, const uint32_t* __restrict__ entries,
-                                                        const uint32_t* __restrict__ offsets, const uint32_t* __restrict__ task_off, uint32_t nb,
-                                                        uint32_t K, const uint32_t* __restrict__ meta, const affine_t* __restrict__ extra,
-                                                        uint32_t main_count, xyzz_t* buckets, xyzz_t* partials) {
-    __shared__ alignas(128) affine_t slots[2][128];
-    __shared__ alignas(8) uint64_t bars[2][4];
-    const unsigned tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t t = blockIdx.x * blockDim.x + tid;
-    if (lane == 0) { mbar_init(smem_u32(&bars[0][warp]), 32); mbar_init(smem_u32(&bars[1][warp]), 32); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    __syncwarp();
-    const bool live = t < __ldg(meta + 1);
-    uint32_t b = 0, sb = 1, i = 0, end = 0;
-    if (live) {
-        uint32_t lo = 0, hi = nb;
-        while (hi - lo > 1) {
-            uint32_t mid = (lo + hi) >> 1;
-            if (__ldg(task_off + mid) <= t) lo = mid; else hi = mid;
-        }
-        b = lo;
-        const uint32_t e0 = __ldg(offsets + b), nbk = __ldg(offsets + b + 1) - e0;
-        sb = (nbk + K - 1) / K;
-        const uint32_t sub = t - __ldg(task_off + b), base = nbk / sb, rem = nbk - base * sb;
-        i = e0 + sub * base + min(sub, rem);
-        end = i + base + (sub < rem ? 1u : 0u);
-    }
-    const uint32_t steps = __reduce_max_sync(0xffffffffu, end - i);
-    uint32_t sign[2] = {0, 0};
-    auto issue = [&](uint32_t step) {
-        const unsigned s = step & 1;
-        const uint32_t bar = smem_u32(&bars[s][warp]);
-        if (i + step < end) {
-            const uint32_t e = __ldg(entries + i + step), idx = e & 0x7fffffffu;
-            sign[s] = e >> 31;
-            // the slot was read with ordinary loads two steps ago: order those (generic proxy) before the copy engine's write
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            mbar_arrive_expect_tx(bar, (uint32_t)sizeof(affine_t));
-            bulk_copy_g2s(smem_u32(&slots[s][tid]), idx < main_count ? points + idx : extra + (idx - main_count), (uint32_t)sizeof(affine_t), bar);
-        } else {
-            mbar_arrive(bar);
-        }
-    };
-    xyzz_t acc = xyzz_identity();
-    if (steps) issue(0);
-    for (uint32_t step = 0; step < steps; step++) {
-        if (step + 1 < steps) issue(step + 1);
-        mbar_wait(smem_u32(&bars[step & 1][warp]), (step >> 1) & 1);
-        if (i + step < end) {
-            const uint4* q4 = reinterpret_cast<const uint4*>(&slots[step & 1][tid]);
-            affine_t q;
-            uint4 v0 = q4[0], v1 = q4[1], v2 = q4[2], v3 = q4[3];
-            q.x.v[0] = v0.x; q.x.v[1] = v0.y; q.x.v[2] = v0.z; q.x.v[3] = v0.w; q.x.v[4] = v1.x; q.x.v[5] = v1.y; q.x.v[6] = v1.z; q.x.v[7] = v1.w;
-            q.y.v[0] = v2.x; q.y.v[1] = v2.y; q.y.v[2] = v2.z; q.y.v[3] = v2.w; q.y.v[4] = v3.x; q.y.v[5] = v3.y; q.y.v[6] = v3.z; q.y.v[7] = v3.w;
-            if (sign[step & 1]) q.y = fe_neg<F>(q.y);
-            acc = xyzz_madd<F>(acc, q);
-        }
-    }
-    if (live) store_xyzz(sb == 1 ? buckets + b : partials + t, acc);
-}
-
 // Balanced first level of the per-bucket sums.  The task partials lie in bucket order; thread u sums the RUN of `run`
 // consecutive partials [u*run, (u+1)*run) segment by segment (a segment = the part of one bucket inside the run) and writes each
 // segment sum back at the segment's first index.  Every thread executes at most run-1 additions whatever the bucket sizes, so a
@@ -574,18 +491,7 @@ __global__ void __launch_bounds__(TREE_THREADS) k_gridsum_final(const xyzz_t* __
     if (threadIdx.x == 0) store_xyzz(out + (size_t)g * c + t, acc);
 }
 
-// ---------------------------------------------------------------------------------------------- workspace
-static void free_dev(void* p) { if (p) cudaFree(p); }
-
-void msm_workspace_free(MsmWorkspace& ws) {
-    free_dev(ws.d_digits); free_dev(ws.d_entries); free_dev(ws.d_partials);
-    free_dev(ws.d_counts); free_dev(ws.d_offsets); free_dev(ws.d_task_off); free_dev(ws.d_buckets); free_dev(ws.d_chain); free_dev(ws.d_chain_flag);
-    free_dev(ws.d_bitsums); free_dev(ws.d_meta); free_dev(ws.d_giants); free_dev(ws.d_giant_slices); free_dev(ws.d_giant_tickets);
-    if (ws.h_bitsums) cudaFreeHost(ws.h_bitsums);
-    for (auto& e : ws.ev) if (e) cudaEventDestroy(e);
-    ws = MsmWorkspace();
-}
-
+// ---------------------------------------------------------------------------------------------- pipeline
 static unsigned pow2_ceil_log(uint64_t x) {
     unsigned l = 0;
     while (((uint64_t)1 << l) < x) l++;
@@ -594,13 +500,14 @@ static unsigned pow2_ceil_log(uint64_t x) {
 
 template <class F, class FS>
 int msm_run(const MsmBases& b, const size_t* offs, size_t n_main, const fe* const* d_scalars, unsigned k, bool scalars_mont, unsigned c,
-            MsmWorkspace& ws, cudaStream_t st, MsmResultShape* shape, unsigned* launches, const affine_t* d_extra, size_t n_extra) {
+            const affine_t* d_extra, size_t n_extra, const MsmTuning& tune, int sm_count, bool profile, MsmWorkspace& ws, cudaStream_t st,
+            xyzz_t* d_out, size_t out_cap, MsmResultShape* shape, unsigned* launches) {
     const size_t n = n_main + n_extra;                // scalars per MSM
     if (n_extra && !d_extra) { zk_set_error("msm: extra points missing"); return ZK_ERR_INVALID; }
     for (unsigned j = 0; j < k && j < MSM_MAX_BATCH; j++)
         if (offs[j] > b.n || n_main > b.n - offs[j]) { zk_set_error("msm: slice [%zu, %zu) outside the %zu resident bases", offs[j], offs[j] + n_main, b.n); return ZK_ERR_INVALID; }
     if (k == 0 || k > MSM_MAX_BATCH) { zk_set_error("msm: batch of %u outside [1, %u]", k, MSM_MAX_BATCH); return ZK_ERR_INVALID; }
-    shape->c = 0; shape->groups = 0; shape->batch = k;
+    shape->c = 0; shape->groups = 0;
     if (n == 0) return ZK_OK;
     const bool use_table = b.c != 0;
     if (use_table) c = b.c;
@@ -609,6 +516,7 @@ int msm_run(const MsmBases& b, const size_t* offs, size_t n_main, const fe* cons
     const unsigned nwin = msm_num_windows(c);
     const unsigned gpm = use_table ? 1 : nwin;        // bucket groups per MSM
     const unsigned G = k * gpm;                       // bucket groups of the batch
+    if (d_out && (size_t)G * c > out_cap) { zk_set_error("msm: %u slice sums do not fit the caller's buffer of %zu points", G * c, out_cap); return ZK_ERR_INVALID; }
     const uint32_t B = 1u << (c - 1);                 // buckets per group
     const size_t NB = (size_t)G * B;
     const size_t Mmax = n * nwin * (size_t)k;
@@ -621,11 +529,11 @@ int msm_run(const MsmBases& b, const size_t* offs, size_t n_main, const fe* cons
     // <= 128 registers); K is chosen so that the tasks fill a whole number of waves (a 1.02-wave grid costs two waves).
     // Short tasks keep the lanes of a warp balanced (a bucket of n_b entries is cut into ceil(n_b / K) equal parts: lengths lie
     // in (K s / (s + 1), K]): one wave of long tasks is slower than two waves of short ones for the same additions.
-    const size_t capacity = (size_t)ws.sm_count * (ws.wave_threads ? ws.wave_threads : 512);
-    const size_t resident_quads = (size_t)ws.sm_count * TREE_QUADS;
+    const size_t capacity = (size_t)sm_count * (tune.wave_threads ? tune.wave_threads : 512);
+    const size_t resident_quads = (size_t)sm_count * TREE_QUADS;
     const bool many_buckets = NB > resident_quads;    // many small buckets: throughput regime (see k_bucket_finish_serial)
     const bool serial_finish = many_buckets;
-    uint32_t K = ws.chunk;
+    uint32_t K = tune.chunk;
     if (K == 0) {
         // (1) lane balance: a bucket of n_b entries is cut into ceil(n_b / K) equal tasks, so task lengths lie in (K s / (s + 1), K];
         //     with s >= 8 tasks per average bucket the lanes of a warp differ by ~10%, whatever the batch size;
@@ -649,132 +557,106 @@ int msm_run(const MsmBases& b, const size_t* offs, size_t n_main, const fe* cons
     const size_t ntiles = (NB + PLAN_TILE - 1) / PLAN_TILE;
 
     static_assert(sizeof(xyzz_t) == 128 && sizeof(affine_t) == 64 && sizeof(fe) == 32, "layout");
-    // scratch, grouped by what sizes it: the entry list (k * n * nwin), the bucket array (G * B), the slice sums (G * c)
-    {
-        const size_t need_entries = Mmax * sizeof(uint32_t), need_partials = NTmax * sizeof(xyzz_t);
-        if (ws.cap_entries < need_entries) {
-            free_dev(ws.d_digits); free_dev(ws.d_entries);
-            ws.d_digits = nullptr; ws.d_entries = nullptr; ws.cap_entries = 0;
-            ZK_CUDA(cudaMalloc(&ws.d_digits, Mmax * sizeof(int32_t)));
-            ZK_CUDA(cudaMalloc(&ws.d_entries, need_entries));
-            ws.cap_entries = need_entries;
-        }
-        if (ws.cap_partials < need_partials) {
-            free_dev(ws.d_partials);
-            ws.d_partials = nullptr; ws.cap_partials = 0;
-            ZK_CUDA(cudaMalloc(&ws.d_partials, need_partials));
-            ws.cap_partials = need_partials;
-        }
-        if (ws.cap_buckets < NB) {
-            free_dev(ws.d_counts); free_dev(ws.d_offsets); free_dev(ws.d_task_off); free_dev(ws.d_buckets); free_dev(ws.d_chain); free_dev(ws.d_chain_flag);
-            ws.d_counts = ws.d_offsets = ws.d_task_off = ws.d_chain_flag = nullptr; ws.d_chain = nullptr; ws.d_buckets = nullptr; ws.cap_buckets = 0;
-            ZK_CUDA(cudaMalloc(&ws.d_counts, NB * sizeof(uint32_t)));
-            ZK_CUDA(cudaMalloc(&ws.d_offsets, (NB + 1) * sizeof(uint32_t)));
-            ZK_CUDA(cudaMalloc(&ws.d_task_off, (NB + 1) * sizeof(uint32_t)));
-            ZK_CUDA(cudaMalloc(&ws.d_buckets, NB * sizeof(xyzz_t)));
-            ZK_CUDA(cudaMalloc(&ws.d_chain, ntiles * sizeof(uint64_t)));
-            ZK_CUDA(cudaMalloc(&ws.d_chain_flag, ntiles * sizeof(uint32_t)));
-            ZK_CUDA(cudaMemsetAsync(ws.d_chain_flag, 0, ntiles * sizeof(uint32_t), st));
-            ws.epoch = 0;
-            ws.cap_buckets = NB;
-        }
-        const size_t need_bits = (size_t)G * (nrows + W) + (size_t)G * c;
-        if (ws.cap_bits < need_bits) {
-            free_dev(ws.d_bitsums);
-            ws.d_bitsums = nullptr; ws.cap_bits = 0;
-            ZK_CUDA(cudaMalloc(&ws.d_bitsums, need_bits * sizeof(xyzz_t)));
-            ws.cap_bits = need_bits;
-        }
-        if (ws.cap_hbits < (size_t)G * c) {   // sized by G*c alone: few wide groups and many narrow ones differ
-            if (ws.defer_sync) ZK_CUDA(cudaStreamSynchronize(st));   // an earlier deferred result may still be in flight
-            if (ws.h_bitsums) cudaFreeHost(ws.h_bitsums);
-            ws.h_bitsums = nullptr; ws.cap_hbits = 0;
-            ZK_CUDA(cudaMallocHost(&ws.h_bitsums, 2 * (size_t)G * c * sizeof(xyzz_t)));
-            ws.cap_hbits = (size_t)G * c;
-        }
-        if (!ws.d_meta) {
-            ZK_CUDA(cudaMalloc(&ws.d_meta, 8 * sizeof(uint32_t)));
-            ZK_CUDA(cudaMalloc(&ws.d_giants, MSM_MAX_GIANTS * sizeof(uint32_t)));
-            ZK_CUDA(cudaMalloc(&ws.d_giant_slices, (size_t)MSM_MAX_GIANTS * GIANT_SLICES * sizeof(xyzz_t)));
-            ZK_CUDA(cudaMalloc(&ws.d_giant_tickets, MSM_MAX_GIANTS * sizeof(uint32_t)));
-            ZK_CUDA(cudaMemsetAsync(ws.d_giant_tickets, 0, MSM_MAX_GIANTS * sizeof(uint32_t), st));
-        }
+    // scratch, grouped by what sizes it (MsmWorkspace)
+    Layout le, lb, lf;
+    const size_t o_digits = le.add(Mmax * sizeof(int32_t)), o_entries = le.add(Mmax * sizeof(uint32_t));
+    const size_t o_counts = lb.add(NB * sizeof(uint32_t)), o_offsets = lb.add((NB + 1) * sizeof(uint32_t)),
+                 o_task_off = lb.add((NB + 1) * sizeof(uint32_t)), o_buckets = lb.add(NB * sizeof(xyzz_t)), o_chain = lb.add(ntiles * sizeof(uint64_t));
+    const size_t o_meta = lf.add(8 * sizeof(uint32_t)), o_giants = lf.add(MSM_MAX_GIANTS * sizeof(uint32_t)),
+                 o_slices = lf.add((size_t)MSM_MAX_GIANTS * GIANT_SLICES * sizeof(xyzz_t)), o_tickets = lf.add(MSM_MAX_GIANTS * sizeof(uint32_t));
+    if (int rc = ws.entries.ensure(le.total)) return rc;
+    if (int rc = ws.partials.ensure(NTmax * sizeof(xyzz_t))) return rc;
+    if (int rc = ws.buckets.ensure(lb.total)) return rc;
+    const size_t flags_had = ws.chain_flags.cap;
+    if (int rc = ws.chain_flags.ensure(ntiles * sizeof(uint32_t))) return rc;
+    if (ws.chain_flags.cap != flags_had) {            // new flags: no stamps yet
+        ZK_CUDA(cudaMemsetAsync(ws.chain_flags.p, 0, ntiles * sizeof(uint32_t), st));
+        ws.epoch = 0;
     }
+    if (int rc = ws.bitsums.ensure(((size_t)G * (nrows + W) + (size_t)G * c) * sizeof(xyzz_t))) return rc;
+    if (!ws.fixed.p) {
+        if (int rc = ws.fixed.ensure(lf.total)) return rc;
+        ZK_CUDA(cudaMemsetAsync(ws.fixed.at<uint32_t>(o_tickets), 0, MSM_MAX_GIANTS * sizeof(uint32_t), st));
+    }
+    if (!d_out)
+        if (int rc = ws.h_bitsums.ensure((size_t)G * c * sizeof(xyzz_t))) return rc;   // sized by G*c alone: few wide groups and many narrow ones differ
+    int32_t* d_digits = ws.entries.at<int32_t>(o_digits);
+    uint32_t* d_entries = ws.entries.at<uint32_t>(o_entries);
+    xyzz_t* d_partials = ws.partials.at<xyzz_t>();
+    uint32_t *d_counts = ws.buckets.at<uint32_t>(o_counts), *d_offsets = ws.buckets.at<uint32_t>(o_offsets), *d_task_off = ws.buckets.at<uint32_t>(o_task_off);
+    xyzz_t* d_buckets = ws.buckets.at<xyzz_t>(o_buckets);
+    uint64_t* d_chain = ws.buckets.at<uint64_t>(o_chain);
+    uint32_t *d_meta = ws.fixed.at<uint32_t>(o_meta), *d_giants = ws.fixed.at<uint32_t>(o_giants), *d_giant_tickets = ws.fixed.at<uint32_t>(o_tickets);
+    xyzz_t* d_giant_slices = ws.fixed.at<xyzz_t>(o_slices);
     unsigned nl = 0;
-    if (ws.profile && !ws.ev[0])
-        for (int s = 0; s <= MSM_ST_COUNT; s++) ZK_CUDA(cudaEventCreate(&ws.ev[s]));
-#define STAGE_MARK(s) do { if (ws.profile) ZK_CUDA(cudaEventRecord(ws.ev[s], st)); } while (0)
+    if (profile && !ws.ev[0].e)
+        for (int s = 0; s <= MSM_ST_COUNT; s++) ZK_CUDA(cudaEventCreate(&ws.ev[s].e));
+#define STAGE_MARK(s) do { if (profile) ZK_CUDA(cudaEventRecord(ws.ev[s].e, st)); } while (0)
 
     MsmScalarSet sc{};
     for (unsigned j = 0; j < k; j++) { sc.p[j] = d_scalars[j]; sc.off[j] = (uint32_t)offs[j]; }
     const uint32_t epoch = ++ws.epoch;
-    ZK_CUDA(cudaMemsetAsync(ws.d_counts, 0, NB * sizeof(uint32_t), st));
-    ZK_CUDA(cudaMemsetAsync(ws.d_buckets, 0, NB * sizeof(xyzz_t), st));  // all-zero XYZZ == identity
+    ZK_CUDA(cudaMemsetAsync(d_counts, 0, NB * sizeof(uint32_t), st));
+    ZK_CUDA(cudaMemsetAsync(d_buckets, 0, NB * sizeof(xyzz_t), st));  // all-zero XYZZ == identity
     STAGE_MARK(0);
     // 1. digits + histogram
-    k_recode<FS><<<dim3((unsigned)((n + 127) / 128), k), 128, 0, st>>>(sc, scalars_mont ? 1 : 0, n, c, nwin, gpm, use_table ? 0 : 1, ws.d_digits,
-                                                                        ws.d_counts, ws.d_meta);
+    k_recode<FS><<<dim3((unsigned)((n + 127) / 128), k), 128, 0, st>>>(sc, scalars_mont ? 1 : 0, n, c, nwin, gpm, use_table ? 0 : 1, d_digits,
+                                                                        d_counts, d_meta);
     STAGE_MARK(1);
     // 2. plan: bucket offsets, task offsets, giant list
-    k_plan<<<(unsigned)ntiles, 1024, 0, st>>>(ws.d_counts, ws.d_offsets, ws.d_task_off, (uint32_t)NB, K, smax, ws.d_meta, ws.d_giants, ws.d_chain,
-                                               ws.d_chain_flag, epoch);
+    k_plan<<<(unsigned)ntiles, 1024, 0, st>>>(d_counts, d_offsets, d_task_off, (uint32_t)NB, K, smax, d_meta, d_giants, d_chain,
+                                               ws.chain_flags.at<uint32_t>(), epoch);
     STAGE_MARK(2);
     // 3. scatter (counting sort by bucket)
-    k_scatter<<<(unsigned)((Mmax + 255) / 256), 256, 0, st>>>(ws.d_digits, n, c, nwin, k, gpm, use_table ? 0 : 1, sc, b.n, use_table ? 1 : 0,
-                                                            n_main, n_extra, (uint32_t)main_count, ws.d_offsets, ws.d_counts, ws.d_entries);
+    k_scatter<<<(unsigned)((Mmax + 255) / 256), 256, 0, st>>>(d_digits, n, c, nwin, k, gpm, use_table ? 0 : 1, sc, b.n, use_table ? 1 : 0,
+                                                            n_main, n_extra, (uint32_t)main_count, d_offsets, d_counts, d_entries);
     STAGE_MARK(3);
     // 4. accumulation: one task per <= K sorted entries of one bucket
-    if (ws.tma_gather)
-        k_accumulate_tma<F><<<(unsigned)((NTmax + 127) / 128), 128, 0, st>>>(b.d_points, ws.d_entries, ws.d_offsets, ws.d_task_off, (uint32_t)NB, K,
-                                                                           ws.d_meta, d_extra, (uint32_t)main_count, ws.d_buckets, ws.d_partials);
-    else
-        k_accumulate<F><<<(unsigned)((NTmax + 127) / 128), 128, 0, st>>>(b.d_points, ws.d_entries, ws.d_offsets, ws.d_task_off, (uint32_t)NB, K, ws.d_meta,
-                                                                       d_extra, (uint32_t)main_count, ws.d_buckets, ws.d_partials);
+    k_accumulate<F><<<(unsigned)((NTmax + 127) / 128), 128, 0, st>>>(b.d_points, d_entries, d_offsets, d_task_off, (uint32_t)NB, K, d_meta,
+                                                                   d_extra, (uint32_t)main_count, d_buckets, d_partials);
     STAGE_MARK(4);
     // 5. per-bucket sums of the task partials (+ giants)
     // giants first: k_giant_finish reads the untouched partial lists, k_run_sum then rewrites partials in place
     k_giant_finish<F><<<dim3(64, GIANT_SLICES), TREE_THREADS, TREE_QUADS * sizeof(xyzz_t), st>>>(
-        ws.d_giants, ws.d_meta, ws.d_offsets, ws.d_task_off, K, ws.d_buckets, ws.d_partials, ws.d_giant_slices, ws.d_giant_tickets);
+        d_giants, d_meta, d_offsets, d_task_off, K, d_buckets, d_partials, d_giant_slices, d_giant_tickets);
     if (serial_finish) {
         const size_t threads = (NTmax + run - 1) / run;
-        k_run_sum<F><<<(unsigned)((threads + 127) / 128), 128, 0, st>>>(ws.d_task_off, (uint32_t)NB, ws.d_meta, run, smax, ws.d_partials);
+        k_run_sum<F><<<(unsigned)((threads + 127) / 128), 128, 0, st>>>(d_task_off, (uint32_t)NB, d_meta, run, smax, d_partials);
         nl += 1;
-        k_bucket_finish_serial<F><<<(unsigned)((NB + 127) / 128), 128, 0, st>>>(ws.d_offsets, ws.d_task_off, (uint32_t)NB, K, smax, ws.d_meta, run, ws.d_buckets, ws.d_partials);
+        k_bucket_finish_serial<F><<<(unsigned)((NB + 127) / 128), 128, 0, st>>>(d_offsets, d_task_off, (uint32_t)NB, K, smax, d_meta, run, d_buckets, d_partials);
     } else {
-        k_bucket_finish<F><<<(unsigned)(((NB << (log_g + 2)) + 127) / 128), 128, 0, st>>>(ws.d_offsets, ws.d_task_off, (uint32_t)NB, K, smax, log_g, ws.d_meta,
-                                                                                  ws.d_buckets, ws.d_partials);
+        k_bucket_finish<F><<<(unsigned)(((NB << (log_g + 2)) + 127) / 128), 128, 0, st>>>(d_offsets, d_task_off, (uint32_t)NB, K, smax, log_g, d_meta,
+                                                                                  d_buckets, d_partials);
     }
     STAGE_MARK(5);
     // 6. two-level bucket reduction: row / column sums of the bucket grid, then their bit slices
-    xyzz_t* d_rc = ws.d_bitsums;
-    xyzz_t* d_T = ws.d_bitsums + (size_t)G * (nrows + W);
+    xyzz_t* d_rc = ws.bitsums.at<xyzz_t>();
+    xyzz_t* d_T = d_rc + (size_t)G * (nrows + W);
     {
         // a quad per 1-4 elements of a row / column, but never more CTAs x threads than are resident at once (384 threads per
         // SM at the kernel's register budget), so that the whole grid of a single MSM — 385 CTAs at window 16 — runs as one wave
         unsigned gt = 128;                          // k_gridsum is built for 3 CTAs of 128 threads per SM (<= 168 registers)
-        while (gt > 32 && (gt / 4 >= 2 * std::max(W, nrows) || (size_t)G * (nrows + W) * gt > (size_t)ws.sm_count * 384)) gt /= 2;
-        k_gridsum<F><<<dim3(nrows + W, 1, G), gt, (gt / 4) * sizeof(xyzz_t), st>>>(ws.d_buckets, B, w_lo, d_rc);
+        while (gt > 32 && (gt / 4 >= 2 * std::max(W, nrows) || (size_t)G * (nrows + W) * gt > (size_t)sm_count * 384)) gt /= 2;
+        k_gridsum<F><<<dim3(nrows + W, 1, G), gt, (gt / 4) * sizeof(xyzz_t), st>>>(d_buckets, B, w_lo, d_rc);
         unsigned ft = TREE_THREADS;                 // half of the elements carry a given bit
         while (ft > 32 && ft / 4 >= std::max(W, nrows)) ft /= 2;
         k_gridsum_final<F><<<dim3(c, G), ft, (ft / 4) * sizeof(xyzz_t), st>>>(d_rc, B, w_lo, c, d_T);
     }
     nl += 8;
     STAGE_MARK(6);
+#undef STAGE_MARK
     ZK_CUDA(cudaGetLastError());
     shape->c = c; shape->groups = gpm;
     if (launches) *launches += nl;
-    if (ws.d_T_out) {
-        if ((size_t)G * c > ws.d_T_cap) { zk_set_error("msm: %u slice sums do not fit the caller's buffer of %zu points", G * c, ws.d_T_cap); return ZK_ERR_INVALID; }
-        ZK_CUDA(cudaMemcpyAsync(ws.d_T_out, d_T, (size_t)G * c * sizeof(xyzz_t), cudaMemcpyDeviceToDevice, st));
+    if (d_out) {
+        ZK_CUDA(cudaMemcpyAsync(d_out, d_T, (size_t)G * c * sizeof(xyzz_t), cudaMemcpyDeviceToDevice, st));
         return ZK_OK;
     }
-    ZK_CUDA(cudaMemcpyAsync(ws.h_bitsums + (size_t)(ws.h_slot & 1) * ws.cap_hbits, d_T, (size_t)G * c * sizeof(xyzz_t), cudaMemcpyDeviceToHost, st));
-    if (ws.defer_sync) return ZK_OK;
+    ZK_CUDA(cudaMemcpyAsync(ws.h_bitsums.p, d_T, (size_t)G * c * sizeof(xyzz_t), cudaMemcpyDeviceToHost, st));
     ZK_CUDA(cudaStreamSynchronize(st));
-    if (ws.profile)
-        for (int s = 0; s < MSM_ST_COUNT; s++) ZK_CUDA(cudaEventElapsedTime(&ws.stage_ms[s], ws.ev[s], ws.ev[s + 1]));
-#undef STAGE_MARK
-    // the O(c) serial tail (c doublings per group) is finished on the host from ws.h_bitsums (api.cu: msm_finish)
+    if (profile)
+        for (int s = 0; s < MSM_ST_COUNT; s++) ZK_CUDA(cudaEventElapsedTime(&ws.stage_ms[s], ws.ev[s].e, ws.ev[s + 1].e));
+    // the O(c) serial tail (c doublings per group) is finished on the host from ws.h_bitsums (api.cu: msm_finish_t)
     return ZK_OK;
 }
 
@@ -805,8 +687,8 @@ template int msm_sum_partials<FqParams>(const xyzz_t*, size_t, size_t, xyzz_t*, 
 
 #define INST(F, FS)                                                                                                             \
     template int msm_bases_create<F>(MsmBases&, const affine_t*, bool, size_t, unsigned, cudaStream_t);                          \
-    template int msm_run<F, FS>(const MsmBases&, const size_t*, size_t, const fe* const*, unsigned, bool, unsigned, MsmWorkspace&, cudaStream_t, MsmResultShape*, unsigned*, \
-                                const affine_t*, size_t);
+    template int msm_run<F, FS>(const MsmBases&, const size_t*, size_t, const fe* const*, unsigned, bool, unsigned, const affine_t*, size_t,          \
+                                const MsmTuning&, int, bool, MsmWorkspace&, cudaStream_t, xyzz_t*, size_t, MsmResultShape*, unsigned*);
 INST(FpParams, FqParams)  // Pallas: coordinates Fp, scalars Fq
 INST(FqParams, FpParams)  // Vesta:  coordinates Fq, scalars Fp
 #undef INST

@@ -48,38 +48,33 @@ struct MsmBases {
     affine_t* d_points = nullptr;  // [max(1,nwin)][n]  row w holds 2^(c*w) * P_i
 };
 
-// Growable device scratch of one context/device (sized for the largest call seen so far).
+// Per-stage device timing of a profiled run (CUDA events on the launching stream).
+enum MsmStage { MSM_ST_RECODE = 0, MSM_ST_PLAN, MSM_ST_SCATTER, MSM_ST_ACCUMULATE, MSM_ST_FINISH, MSM_ST_BITSUM, MSM_ST_COUNT };
+
+// Device scratch of one lane's pipeline, sized for the largest call seen so far, grouped by what sizes it (M sorted entries, NB
+// buckets in G groups of B, `tiles` scan tiles of k_plan, K entries per task).
 struct MsmWorkspace {
-    size_t cap_entries = 0, cap_partials = 0, cap_buckets = 0, cap_bits = 0, cap_hbits = 0;
-    int32_t* d_digits = nullptr;      // [k][nwin][n]
-    uint32_t* d_entries = nullptr;    // [M]  point index | sign << 31, sorted by bucket
-    xyzz_t* d_partials = nullptr;     // [tasks] one partial sum per accumulation task
-    uint32_t* d_counts = nullptr;     // [NB]     histogram, then scatter cursors
-    uint32_t* d_offsets = nullptr;    // [NB + 1] exclusive scan of the counts
-    uint32_t* d_task_off = nullptr;   // [NB + 1] exclusive scan of ceil(count / K)
-    xyzz_t* d_buckets = nullptr;      // [NB]
-    uint64_t* d_chain = nullptr;      // [tiles] chained scan of k_plan: inclusive (entries << 32 | tasks) per tile
-    uint32_t* d_chain_flag = nullptr; // [tiles] epoch stamps of d_chain
-    uint32_t epoch = 0;               // bumped per run (no flag memset)
-    xyzz_t* d_bitsums = nullptr;      // row/column sums [G][nrows + W], then the slice sums [G][c]
-    xyzz_t* h_bitsums = nullptr;      // pinned host copies of [G][c]: two slots (a lane may run ahead of the host tail by one MSM)
-    unsigned h_slot = 0;              // slot the next msm_run writes (result at h_bitsums + h_slot * cap_hbits)
-    xyzz_t* d_T_out = nullptr;        // when set: the slice sums are copied HERE (device, capacity d_T_cap points) instead of to
-    size_t d_T_cap = 0;               // the host, and nothing is synchronised (multi-GPU exchange, zk_msm_partial)
-    bool defer_sync = false;          // msm_run returns after enqueueing the D2H copy; the caller synchronises
-    uint32_t* d_meta = nullptr;       // [0] sorted entries, [1] tasks, [2] giant buckets
-    uint32_t* d_giants = nullptr;     // [MSM_MAX_GIANTS] bucket ids
-    xyzz_t* d_giant_slices = nullptr; // [MSM_MAX_GIANTS][GIANT_SLICES] per-CTA slice sums of a giant's partials
-    uint32_t* d_giant_tickets = nullptr;  // [MSM_MAX_GIANTS] arrival counters (self-resetting)
-    uint32_t chunk = 0;               // K override (0: chosen per call so that the tasks fill the machine once)
-    uint32_t wave_threads = 0;        // accumulation threads per SM the task count is sized for (0: built-in default)
-    bool tma_gather = false;          // A/B switch: gather the points with the bulk asynchronous copy engine (k_accumulate_tma)
-    int sm_count = 132;               // SMs of the device (set by the context)
-    bool profile = false;             // record an event after every stage
-    cudaEvent_t ev[8] = {};           // MSM_ST_COUNT + 1 stage boundaries
-    float stage_ms[8] = {};           // duration of each stage in the last profiled call
+    DevScratch entries;        // digits int32[M] | entries u32[M]: point index | sign << 31, sorted by bucket
+    DevScratch partials;       // xyzz_t[M / K + NB + 1]: one partial sum per accumulation task
+    DevScratch buckets;        // counts u32[NB]: histogram, then scatter cursors | offsets, task offsets u32[NB + 1]: exclusive scans
+                               // of the counts and of ceil(count / K) | xyzz_t[NB] | chain u64[tiles]: inclusive (entries << 32 | tasks)
+    DevScratch chain_flags;    // u32[tiles]: epoch stamps of the chain; an allocation of their own, so that no other array of a
+                               // differently sized run ever lands on a stamp slot
+    DevScratch bitsums;        // row/column sums xyzz_t[G][nrows + W], then the slice sums [G][c]
+    DevScratch fixed;          // meta u32[8]: [0] sorted entries, [1] tasks, [2] giant buckets | giant bucket ids u32[MSM_MAX_GIANTS] |
+                               // per-CTA slice sums of a giant's partials | arrival tickets u32[MSM_MAX_GIANTS] (self-resetting)
+    PinnedScratch h_bitsums;   // host copy of the slice sums [G][c]
+    uint32_t epoch = 0;        // stamp of the chain flags, bumped per run (no flag memset)
+    Event ev[MSM_ST_COUNT + 1];         // stage boundaries of a profiled run
+    float stage_ms[MSM_ST_COUNT] = {};  // duration of each stage in the last profiled call
 };
-void msm_workspace_free(MsmWorkspace& ws);
+
+// zk_ctx_set_option's MSM settings; every lane of a context runs with those of its primary lane
+struct MsmTuning {
+    int batch = (int)MSM_MAX_BATCH;   // "msm_batch": MSMs of one call fused into one pipeline
+    uint32_t chunk = 0;               // "msm_chunk": entries per task (0: chosen per call so that the tasks fill the machine once)
+    uint32_t wave_threads = 0;        // "msm_wave_threads": accumulation threads per SM the task count is sized for (0: built-in default)
+};
 
 int msm_default_window(size_t n, bool precomputed);
 unsigned msm_num_windows(unsigned c);
@@ -88,28 +83,26 @@ unsigned msm_num_windows(unsigned c);
 template <class F> int msm_bases_create(MsmBases& b, const affine_t* pts, bool pts_on_device, size_t n, unsigned c_table, cudaStream_t st);
 void msm_bases_free(MsmBases& b);
 
-// Optional per-stage device timing (CUDA events on the launching stream), filled when MsmWorkspace::profile is set.
-enum MsmStage { MSM_ST_RECODE = 0, MSM_ST_PLAN, MSM_ST_SCATTER, MSM_ST_ACCUMULATE, MSM_ST_FINISH, MSM_ST_BITSUM, MSM_ST_COUNT };
-
-// What msm_run leaves in ws.h_bitsums: batch x groups x c XYZZ points T[j][g][t]; MSM j is sum_g 2^(c g) sum_t 2^t T[j][g][t].
+// What msm_run leaves in ws.h_bitsums (or at d_out): k x groups x c XYZZ points T[j][g][t]; MSM j is sum_g 2^(c g) sum_t 2^t T[j][g][t].
 struct MsmResultShape {
     unsigned c = 0, groups = 0;   // groups == 0: empty MSM (identity)
-    unsigned batch = 0;
 };
 
-// k <= MSM_MAX_BATCH MSMs in one pipeline, MSM j over bases[offs[j] .. offs[j]+n).  d_scalars[j]: the n scalars of MSM j, already on the device
-// (8 u32 each).  window c: 0 = default (ignored when the bases carry a precomputed table).  Synchronises the stream (unless
-// ws.defer_sync / ws.d_T_out); the O(c) tail is finished by the caller.
-// d_extra / n_extra: n_extra further points that belong to this call only (h and the fresh base U of an IPA round,
-// poly-commitment/src/ipa.rs:944,954), laid out like the table — row w holds 2^(c*w) * E_e at d_extra[w * n_extra + e] (one row
-// without a table); every scalar vector then carries n_main + n_extra scalars, the extras' last.
 // out[i] = sum over r < world of all[r * count + i]   (the cross-rank sum of gathered slice sums, i < count)
 template <class F> int msm_sum_partials(const xyzz_t* d_all, size_t world, size_t count, xyzz_t* d_out, cudaStream_t st);
 
+// k <= MSM_MAX_BATCH MSMs in one pipeline, MSM j over bases[offs[j] .. offs[j]+n).  d_scalars[j]: the n scalars of MSM j, already on the device
+// (8 u32 each).  window c: 0 = default (ignored when the bases carry a precomputed table).  The O(c) tail is finished by the caller.
+// d_extra / n_extra: n_extra further points that belong to this call only (h and the fresh base U of an IPA round,
+// poly-commitment/src/ipa.rs:944,954), laid out like the table — row w holds 2^(c*w) * E_e at d_extra[w * n_extra + e] (one row
+// without a table); every scalar vector then carries n_main + n_extra scalars, the extras' last.
+// d_out null: the slice sums are copied to ws.h_bitsums and the stream is synchronised (with `profile`, ws.stage_ms is filled).
+// Otherwise they are copied to d_out (device, room for out_cap points; refused before anything runs when too small) and nothing
+// is synchronised (multi-GPU exchange, zk_msm_partial).  sm_count: SMs of the device.
 template <class F, class FS>
 int msm_run(const MsmBases& b, const size_t* offs, size_t n_main, const fe* const* d_scalars, unsigned k, bool scalars_mont, unsigned c,
-            MsmWorkspace& ws, cudaStream_t st, MsmResultShape* shape, unsigned* launches, const affine_t* d_extra = nullptr,
-            size_t n_extra = 0);
+            const affine_t* d_extra, size_t n_extra, const MsmTuning& tune, int sm_count, bool profile, MsmWorkspace& ws, cudaStream_t st,
+            xyzz_t* d_out, size_t out_cap, MsmResultShape* shape, unsigned* launches);
 
 // group_ntt.cu: Lagrange-basis commitments of the domain of size 2^log_n from the resident generators (SRS::lagrange_basis)
 template <class F, class FS> int lagrange_basis_build(const MsmBases& g, unsigned log_n, unsigned chunk, affine_t* d_out, cudaStream_t st, unsigned* launches);

@@ -133,20 +133,17 @@ def test_sparse_and_short_scalars(ctx, orc, vesta_srs, sparsity, bitlen):
 
 
 @pytest.mark.parametrize("wb", [-1, 0, 9])
-def test_tma_staged_gather_gives_the_same_points(ctx, orc, vesta_srs, wb):
-    """the A/B option of tools/msm_tma_ab.py: accumulation with the gather on the bulk copy engine (option msm_tma) returns
-    what the default kernel and the oracle return — tables, plain bases, and the degenerate one-bucket column"""
+def test_random_and_all_ones_scalars_vs_oracle(ctx, orc, vesta_srs, wb):
+    """random scalars and the degenerate one-bucket column against the oracle: the default table, plain bases and a window-9 table"""
     srs = vesta_srs
     n = 3000
     sc = orc.random_scalars(srs.scalar, n, seed=77)
     ones = np.zeros((n, 4), dtype=np.uint64); ones[:, 0] = 1
     bases = ctx.upload_bases(srs.cid, srs.g[:n], window_bits=wb)
     try:
-        ctx.set_option("msm_tma", 1)
         for scal in (sc, ones):
             assert np.array_equal(ctx.msm_affine(bases, scal), orc.msm(srs.cid, srs.g[:n], scal))
     finally:
-        ctx.set_option("msm_tma", 0)
         bases.free()
 
 
@@ -259,6 +256,8 @@ def test_error_codes(ctx, orc, pallas_srs):
         ctx.ntt(5, np.zeros((4, 4), dtype=np.uint64))  # unknown field id
     with pytest.raises(zk.ZkError):
         ctx.ntt_dev(zk.FP, 0, 21)                      # log_n beyond the two-pass plan
+    with pytest.raises(zk.ZkError):
+        ctx.set_option("msm_tma", 1)                   # unknown option
     other = zk.Context(0)
     with pytest.raises(zk.ZkError):
         other.msm(bases, sc)                           # bases belong to another context
@@ -294,8 +293,10 @@ def test_partial_and_finish_gathered_emulate_two_ranks(ctx, orc, vesta_srs):
         assert ctx.msm_partial(bases, h_sc.data_ptr() + 32 * half, half, packed[1].data_ptr(), cnt, off=half, window_bits=w) == (c, g)
         two = ctx.msm_finish_gathered(srs.cid, packed.data_ptr(), 2, c, g)
         assert np.array_equal(zk.jacobian_to_affine(srs.cid, two), want), wb
+        launched = ctx.launch_count
         with pytest.raises(zk.ZkError):
             ctx.msm_partial(bases, d_sc.data_ptr(), n, d_all.data_ptr(), 1)      # buffer too small for the slice sums
+        assert ctx.launch_count == launched                                       # refused before anything runs
         bases.free()
 
 

@@ -7,8 +7,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import proof_systems_b200 as zk
 from bench import splitmix64_limbs
-tma_ab = len(sys.argv) > 1 and sys.argv[1] == "msm_tma"      # alternate the two accumulate kernels
-if tma_ab: sys.argv[1] = "16"
 wb = int(sys.argv[1]) if len(sys.argv) > 1 else 16
 reps = int(sys.argv[2]) if len(sys.argv) > 2 else 3
 ctx = zk.Context(0)
@@ -19,8 +17,7 @@ d = torch.from_numpy(splitmix64_limbs(1, 1 << 16).view(np.int64)).cuda()
 p20 = torch.from_numpy(splitmix64_limbs(2, 1 << 20).view(np.int64)).cuda()
 p16 = torch.from_numpy(splitmix64_limbs(2, 1 << 16).view(np.int64)).cuda()
 flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
-for it in range(2 * reps if tma_ab else reps):
-    if tma_ab: ctx.set_option("msm_tma", it & 1)
+for it in range(reps):
     flush.fill_(1); torch.cuda.synchronize()
     ctx.msm_dev(bases, d.data_ptr(), 1 << 16)
     flush.fill_(1); torch.cuda.synchronize()
