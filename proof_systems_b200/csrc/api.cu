@@ -157,21 +157,23 @@ int ctx_msm_finish_gathered(zk_ctx* ctx, int curve_id, const void* d_all, size_t
 }
 
 static int ctx_side_streams_init(zk_ctx* ctx) {
-    if (ctx->ev_fork) return ZK_OK;
-    for (int l = 0; l < zk_ctx::SIDE_STREAMS; l++) ZK_CUDA(cudaStreamCreateWithFlags(&ctx->side[l], cudaStreamNonBlocking));
-    ZK_CUDA(cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming));
+    for (Stream& s : ctx->side) ZK_CUDA(s.create(cudaStreamNonBlocking));
+    ZK_CUDA(ctx->ev_fork.create(cudaEventDisableTiming));
     return ZK_OK;
 }
 
+// Tables are built in a local owner and enter the cache only once complete: a failed build leaves no entry behind.
 static int ctx_ntt_tables(zk_ctx* lane, int field, unsigned log_n, bool inverse, const fe** small, const NttTables** tabs) {
     zk_ctx* ctx = ctx_root(lane);                      // one cache per pool; entries are immutable once built
     std::lock_guard<std::mutex> tl(ctx->tab_mu);
-    fe*& sm = ctx->ntt_small[field][inverse ? 1 : 0];
-    if (!sm) {
-        ZK_CUDA(cudaMalloc(&sm, 512 * sizeof(fe)));
-        int rc = with_field(field, [&](auto f) { return ntt_build_small_table<typename decltype(f)::Dev>(sm, inverse, lane->stream); });
+    DevScratch& sm = ctx->ntt_small[field][inverse ? 1 : 0];
+    if (!sm.p) {
+        DevScratch t;
+        if (int rc = t.ensure(512 * sizeof(fe))) return rc;
+        int rc = with_field(field, [&](auto f) { return ntt_build_small_table<typename decltype(f)::Dev>(t.at<fe>(), inverse, lane->stream); });
         if (rc) return rc;
         lane->launches += 2;
+        sm = std::move(t);
     }
     unsigned key = (unsigned)field | (inverse ? 2u : 0u) | (log_n << 2);
     auto it = ctx->ntt_tables.find(key);
@@ -179,10 +181,10 @@ static int ctx_ntt_tables(zk_ctx* lane, int field, unsigned log_n, bool inverse,
         NttTables t;
         int rc = with_field(field, [&](auto f) { return ntt_build_tables<typename decltype(f)::Dev>(t, log_n, inverse, lane->stream); });
         if (rc) return rc;
-        lane->launches += t.full ? 8 : 7;
-        it = ctx->ntt_tables.emplace(key, t).first;
+        lane->launches += t.full.p ? 8 : 7;
+        it = ctx->ntt_tables.emplace(key, std::move(t)).first;
     }
-    *small = sm;
+    *small = sm.at<fe>();
     *tabs = &it->second;
     return ZK_OK;
 }
@@ -220,17 +222,17 @@ int ctx_ntt_device_oop(zk_ctx* ctx, int field, const fe* d_in, size_t in_bs, fe*
     }
     unsigned nl = 0;
     if (ctx->profile) {
-        if (!ctx->ev_ntt[0]) { ZK_CUDA(cudaEventCreate(&ctx->ev_ntt[0])); ZK_CUDA(cudaEventCreate(&ctx->ev_ntt[1])); }
-        ZK_CUDA(cudaEventRecord(ctx->ev_ntt[0], ctx->stream));
+        for (Event& ev : ctx->ev_ntt) ZK_CUDA(ev.create(cudaEventDefault));
+        ZK_CUDA(cudaEventRecord(ctx->ev_ntt[0].e, ctx->stream));
     }
     rc = with_field(field, [&](auto f) {
         return ntt_run<typename decltype(f)::Dev>(d_in, in_bs, d_out, tmp, small, *tabs, inner, log_n, batch, in_len, inverse != 0, coset != 0, ctx->stream, &nl);
     });
     ctx->launches += nl;
     if (rc == ZK_OK && ctx->profile) {
-        ZK_CUDA(cudaEventRecord(ctx->ev_ntt[1], ctx->stream));
-        ZK_CUDA(cudaEventSynchronize(ctx->ev_ntt[1]));
-        ZK_CUDA(cudaEventElapsedTime(&ctx->ntt_ms, ctx->ev_ntt[0], ctx->ev_ntt[1]));
+        ZK_CUDA(cudaEventRecord(ctx->ev_ntt[1].e, ctx->stream));
+        ZK_CUDA(cudaEventSynchronize(ctx->ev_ntt[1].e));
+        ZK_CUDA(cudaEventElapsedTime(&ctx->ntt_ms, ctx->ev_ntt[0].e, ctx->ev_ntt[1].e));
     }
     return rc;
 }
@@ -242,16 +244,16 @@ int ctx_ntt_device(zk_ctx* ctx, int field, fe* d_data, unsigned log_n, size_t ba
 // ---------------------------------------------------------------------------------------------- lanes
 static int ctx_init_lane(zk_ctx* c, int device_id) {
     c->device = device_id;
-    cudaError_t se = cudaStreamCreateWithFlags(&c->own_stream, cudaStreamNonBlocking);
+    cudaError_t se = c->own_stream.create(cudaStreamNonBlocking);
     if (se != cudaSuccess) { zk_set_error("cudaStreamCreate: %s", cudaGetErrorString(se)); return ZK_ERR_CUDA; }
-    c->stream = c->own_stream;
+    c->stream = c->own_stream.s;
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device_id) == cudaSuccess) c->sm_count = prop.multiProcessorCount;
     return ZK_OK;
 }
 
 // host-pointer calls share the lane pool only on the own stream, unprofiled, with more than one lane (ctx->mu held)
-static void ctx_update_pinned(zk_ctx* ctx) { ctx->pinned = ctx->stream != ctx->own_stream || ctx->profile || ctx->n_lanes <= 1; }
+static void ctx_update_pinned(zk_ctx* ctx) { ctx->pinned = ctx->stream != ctx->own_stream.s || ctx->profile || ctx->n_lanes <= 1; }
 
 int ctx_acquire_lane(zk_ctx* ctx, LaneLock& out) {
     ctx = ctx_root(ctx);
@@ -271,14 +273,14 @@ int ctx_acquire_lane(zk_ctx* ctx, LaneLock& out) {
     {
         std::lock_guard<std::mutex> pl(ctx->pool_mu);
         while ((int)ctx->children.size() + 1 < ctx->n_lanes) {
-            zk_ctx* c = new zk_ctx();
+            auto c = std::make_unique<zk_ctx>();
             c->parent = ctx;
-            if (cudaSetDevice(ctx->device) != cudaSuccess || ctx_init_lane(c, ctx->device) != ZK_OK) { delete c; break; }
+            if (cudaSetDevice(ctx->device) != cudaSuccess || ctx_init_lane(c.get(), ctx->device) != ZK_OK) break;
             c->msm = ctx->msm;
-            ctx->children.push_back(c);
+            ctx->children.push_back(std::move(c));
         }
         lanes.push_back(ctx);
-        lanes.insert(lanes.end(), ctx->children.begin(), ctx->children.end());
+        for (auto& c : ctx->children) lanes.push_back(c.get());
         start = ctx->rr++;
     }
     // the primary lane first, then the children in order: a single-threaded caller always lands on the same (warm) lane, only
@@ -374,40 +376,29 @@ int zk_ctx_create(int device_id, zk_ctx** out) {
     }
     if (device_id < 0 || device_id >= n) { zk_set_error("ctx_create: device %d outside [0, %d)", device_id, n); return ZK_ERR_INVALID; }
     ZK_CUDA(cudaSetDevice(device_id));
-    zk_ctx* ctx = new zk_ctx();
-    if (int rc = ctx_init_lane(ctx, device_id)) { delete ctx; return rc; }
-    *out = ctx;
+    auto ctx = std::make_unique<zk_ctx>();
+    if (int rc = ctx_init_lane(ctx.get(), device_id)) return rc;
+    *out = ctx.release();
     return ZK_OK;
 }
 
 void zk_ctx_destroy(zk_ctx* ctx) {
     if (!ctx) return;
-    for (zk_ctx* c : ctx->children) zk_ctx_destroy(c);
-    ctx->children.clear();
     cudaSetDevice(ctx->device);
-    cudaStreamSynchronize(ctx->stream);
-    for (int l = 0; l < zk_ctx::SIDE_STREAMS; l++)
-        if (ctx->side[l]) { cudaStreamSynchronize(ctx->side[l]); cudaStreamDestroy(ctx->side[l]); }
-    if (ctx->ev_fork) cudaEventDestroy(ctx->ev_fork);
-    if (ctx->ev_switch) cudaEventDestroy(ctx->ev_switch);
-    for (int f = 0; f < 2; f++) for (int d = 0; d < 2; d++) if (ctx->ntt_small[f][d]) cudaFree(ctx->ntt_small[f][d]);
-    for (auto& kv : ctx->ntt_tables) ntt_free_tables(kv.second);
-    for (auto& e : ctx->ev_ntt) if (e) cudaEventDestroy(e);
-    cudaStreamDestroy(ctx->own_stream);
-    delete ctx;                          // frees the scratch members on this device
+    delete ctx;                          // ~zk_ctx: the lanes wait for their streams, then everything they own is freed on this device
 }
 
 int zk_ctx_set_stream(zk_ctx* ctx, void* cuda_stream) {
     if (!ctx) { zk_set_error("set_stream: ctx is null"); return ZK_ERR_INVALID; }
     std::lock_guard<std::mutex> lk(ctx->mu);
-    cudaStream_t next = cuda_stream ? (cudaStream_t)cuda_stream : ctx->own_stream;
+    cudaStream_t next = cuda_stream ? (cudaStream_t)cuda_stream : ctx->own_stream.s;
     if (next == ctx->stream) return ZK_OK;
     // Several calls return with kernels still queued that read the context's scratch (the NTT's second buffer, the expression
     // program, the MSM workspace, ...).  The new stream waits for everything queued on the old one so far, without blocking the host.
     ZK_CUDA(cudaSetDevice(ctx->device));
-    if (!ctx->ev_switch) ZK_CUDA(cudaEventCreateWithFlags(&ctx->ev_switch, cudaEventDisableTiming));
-    ZK_CUDA(cudaEventRecord(ctx->ev_switch, ctx->stream));
-    ZK_CUDA(cudaStreamWaitEvent(next, ctx->ev_switch, 0));
+    ZK_CUDA(ctx->ev_switch.create(cudaEventDisableTiming));
+    ZK_CUDA(cudaEventRecord(ctx->ev_switch.e, ctx->stream));
+    ZK_CUDA(cudaStreamWaitEvent(next, ctx->ev_switch.e, 0));
     ctx->stream = next;
     ctx_update_pinned(ctx);
     return ZK_OK;
@@ -416,7 +407,7 @@ int zk_ctx_set_stream(zk_ctx* ctx, void* cuda_stream) {
 uint64_t zk_ctx_launch_count(const zk_ctx* ctx) {
     if (!ctx) return 0;
     uint64_t n = ctx->launches;
-    for (const zk_ctx* c : ctx->children) n += c->launches;
+    for (const auto& c : ctx->children) n += c->launches;
     return n;
 }
 
@@ -450,7 +441,7 @@ int zk_ctx_set_option(zk_ctx* ctx, const char* name, long value) {
         zk_set_error("set_option: unknown option '%s'", name);
         return ZK_ERR_INVALID;
     }
-    for (zk_ctx* c : ctx->children) c->msm = ctx->msm;
+    for (auto& c : ctx->children) c->msm = ctx->msm;
     return ZK_OK;
 }
 
@@ -470,13 +461,13 @@ int zk_bases_upload(zk_ctx* ctx, int curve_id, const uint64_t* xy_mont, size_t n
     std::lock_guard<std::mutex> lk(ctx->mu);
     ZK_CUDA(cudaSetDevice(ctx->device));
     unsigned c = window_bits < 0 ? (unsigned)msm_default_window(n, true) : (unsigned)window_bits;
-    zk_bases* bs = new zk_bases();
+    auto bs = std::make_unique<zk_bases>();
     bs->ctx = ctx;
     bs->b.curve = curve_id;
     int rc = with_curve(curve_id, [&](auto cv) { return msm_bases_create<typename decltype(cv)::F>(bs->b, (const affine_t*)xy_mont, points_on_device != 0, n, c, ctx->stream); });
-    if (rc) { msm_bases_free(bs->b); delete bs; return rc; }
+    if (rc) return rc;
     if (c) ctx->launches += 1;
-    *out = bs;
+    *out = bs.release();
     return ZK_OK;
 }
 
@@ -484,7 +475,6 @@ void zk_bases_free(zk_bases* bases) {
     if (!bases) return;
     std::lock_guard<std::mutex> lk(bases->ctx->mu);
     cudaSetDevice(bases->ctx->device);
-    msm_bases_free(bases->b);
     delete bases;
 }
 
@@ -717,31 +707,30 @@ int zk_ntt_batch(zk_ctx* root, int field_id, uint64_t* data, unsigned log_n, siz
     }
     rc = ctx_side_streams_init(ctx);
     if (rc) return rc;
-    cudaStream_t s_in = ctx->side[0], s_out = ctx->side[1];
+    cudaStream_t s_in = ctx->side[0].s, s_out = ctx->side[1].s;
     const size_t chunks = (batch + per - 1) / per;
-    std::vector<cudaEvent_t> ev(2 * chunks, nullptr);
-    cudaError_t e = cudaEventRecord(ctx->ev_fork, ctx->stream);      // work already queued on the caller's stream comes first
-    if (e == cudaSuccess) e = cudaStreamWaitEvent(s_in, ctx->ev_fork, 0);
+    std::vector<Event> ev(2 * chunks);
+    cudaError_t e = cudaEventRecord(ctx->ev_fork.e, ctx->stream);    // work already queued on the caller's stream comes first
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(s_in, ctx->ev_fork.e, 0);
     for (size_t k = 0; k < chunks && e == cudaSuccess && rc == ZK_OK; k++) {
         const size_t j0 = k * per, cnt = std::min(per, batch - j0);
         fe* d = d_ntt + j0 * n;
         const uint64_t* h = data + 4 * j0 * n;
-        e = cudaEventCreateWithFlags(&ev[2 * k], cudaEventDisableTiming);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev[2 * k + 1], cudaEventDisableTiming);
+        e = ev[2 * k].create(cudaEventDisableTiming);
+        if (e == cudaSuccess) e = ev[2 * k + 1].create(cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaMemcpy2DAsync(d, poly_bytes, h, poly_bytes, in_len * sizeof(fe), cnt, cudaMemcpyHostToDevice, s_in);
-        if (e == cudaSuccess) e = cudaEventRecord(ev[2 * k], s_in);
-        if (e == cudaSuccess) e = cudaStreamWaitEvent(ctx->stream, ev[2 * k], 0);
+        if (e == cudaSuccess) e = cudaEventRecord(ev[2 * k].e, s_in);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(ctx->stream, ev[2 * k].e, 0);
         if (e != cudaSuccess) break;
         rc = ctx_ntt_device(ctx, field_id, d, log_n, cnt, in_len, inverse, coset);
         if (rc) break;
-        e = cudaEventRecord(ev[2 * k + 1], ctx->stream);
-        if (e == cudaSuccess) e = cudaStreamWaitEvent(s_out, ev[2 * k + 1], 0);
+        e = cudaEventRecord(ev[2 * k + 1].e, ctx->stream);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(s_out, ev[2 * k + 1].e, 0);
         if (e == cudaSuccess) e = cudaMemcpyAsync((void*)h, d, cnt * poly_bytes, cudaMemcpyDeviceToHost, s_out);
     }
     cudaStreamSynchronize(s_in);
     cudaStreamSynchronize(ctx->stream);
     cudaError_t e2 = cudaStreamSynchronize(s_out);
-    for (auto& x : ev) if (x) cudaEventDestroy(x);
     if (rc) return rc;
     if (e != cudaSuccess || e2 != cudaSuccess) { zk_set_error("ntt: %s", cudaGetErrorString(e != cudaSuccess ? e : e2)); return ZK_ERR_CUDA; }
     return ZK_OK;
@@ -783,8 +772,8 @@ int zk_debug_op_throughput(zk_ctx* ctx, int field_id, int kind, unsigned blocks,
     if (int rc = dout.ensure(sizeof(xyzz_t))) return rc;
     xyzz_t* d = dout.at<xyzz_t>();
     Event e0, e1;
-    ZK_CUDA(cudaEventCreate(&e0.e));
-    ZK_CUDA(cudaEventCreate(&e1.e));
+    ZK_CUDA(e0.create(cudaEventDefault));
+    ZK_CUDA(e1.create(cudaEventDefault));
     for (int rep = 0; rep < 2; rep++) {  // first launch warms up
         ZK_CUDA(cudaEventRecord(e0.e, ctx->stream));
         with_field(field_id, [&](auto f) {

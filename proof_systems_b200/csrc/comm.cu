@@ -64,10 +64,11 @@ int nccl_check(ncclResult_t r, const char* what) {
 
 struct zk_comm {
     zk_ctx* ctx = nullptr;
-    ncclComm_t comm = nullptr;
+    ncclComm_t comm = nullptr;        // NCCL's handle: destroyed explicitly by zk_comm_destroy
     int world = 1, rank = 0;
-    zkb::xyzz_t* d_mine = nullptr;    // this rank's slice sums
-    zkb::xyzz_t* d_all = nullptr;     // world x slice sums
+    zkb::DevScratch slices;           // this rank's slice sums | world x slice sums
+    zkb::xyzz_t* d_mine = nullptr;
+    zkb::xyzz_t* d_all = nullptr;
     size_t cap_points = 0;
 };
 
@@ -89,25 +90,22 @@ int zk_comm_init_rank(zk_ctx* ctx, const uint8_t id[128], int world, int rank, z
     if (!nccl().ok) { zk_set_error("comm: libnccl.so.2 could not be loaded"); return ZK_ERR_INVALID; }
     std::lock_guard<std::mutex> lk(ctx->mu);
     ZK_CUDA(cudaSetDevice(ctx->device));
-    zk_comm* c = new zk_comm();
+    auto c = std::make_unique<zk_comm>();
     c->ctx = ctx; c->world = world; c->rank = rank;
     ncclUniqueId uid;
     memcpy(uid.internal, id, 128);
     int rc = nccl_check(nccl().CommInitRank(&c->comm, world, uid, rank), "ncclCommInitRank");
-    if (rc) { delete c; return rc; }
-    *out = c;
+    if (rc) return rc;
+    *out = c.release();
     return ZK_OK;
 }
 
 void zk_comm_destroy(zk_comm* c) {
     if (!c) return;
-    {
-        std::lock_guard<std::mutex> lk(c->ctx->mu);
-        cudaSetDevice(c->ctx->device);
-        cudaStreamSynchronize(c->ctx->stream);
-        if (c->comm) nccl().CommDestroy(c->comm);
-        if (c->d_mine) cudaFree(c->d_mine);
-    }
+    std::lock_guard<std::mutex> lk(c->ctx->mu);
+    cudaSetDevice(c->ctx->device);
+    cudaStreamSynchronize(c->ctx->stream);
+    if (c->comm) nccl().CommDestroy(c->comm);
     delete c;
 }
 
@@ -125,7 +123,8 @@ int zk_msm_sharded(zk_comm* c, const zk_bases* bases, size_t off, size_t n, cons
     ZK_CUDA(cudaSetDevice(ctx->device));
     constexpr size_t MAX_POINTS = 4096;       // groups x c of any supported window
     if (!c->d_mine) {
-        ZK_CUDA(cudaMalloc(&c->d_mine, (1 + (size_t)c->world) * MAX_POINTS * sizeof(xyzz_t)));
+        if (int rc = c->slices.ensure((1 + (size_t)c->world) * MAX_POINTS * sizeof(xyzz_t))) return rc;
+        c->d_mine = c->slices.at<xyzz_t>();
         c->d_all = c->d_mine + MAX_POINTS;
         c->cap_points = MAX_POINTS;
     }

@@ -1,9 +1,10 @@
-// common.cuh — error handling, self-freeing scratch memory and events, vectorised element access, library-wide ids.
+// common.cuh — error handling, the owners of device memory, streams and events, vectorised element access, library-wide ids.
 #pragma once
 #include <cuda_runtime.h>
 
 #include <cstdint>
 #include <cstdio>
+#include <utility>
 
 #include "../../include/zkb200.h"
 #include "curve.cuh"
@@ -22,14 +23,19 @@ void zk_set_error(const char* fmt, ...);
         }                                                                                  \
     } while (0)
 
-// Memory that grows on demand (the contents are not kept) and is freed with its owner: device memory, or page-locked host memory
-// with PINNED.  zk_ctx_destroy makes the context's device current before its members are destroyed.
+// The library's device memory, streams and events live in the owners below and are released with them; only zk_dev_alloc's memory
+// belongs to the caller.  Whoever destroys an owner makes its device current first (zk_ctx_destroy and the handles' free functions).
+
+// Memory that grows on demand (the contents are not kept): device memory, or page-locked host memory with PINNED.  Moving hands the
+// buffer over, so a table built in a local owner is published to a cache only once it is complete.
 template <bool PINNED> struct Scratch {
     void* p = nullptr;
     size_t cap = 0;
     Scratch() = default;
     Scratch(const Scratch&) = delete;
     Scratch& operator=(const Scratch&) = delete;
+    Scratch(Scratch&& o) noexcept : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)) {}
+    Scratch& operator=(Scratch&& o) noexcept { std::swap(p, o.p), std::swap(cap, o.cap); return *this; }   // the old buffer leaves with o
     ~Scratch() { release(); }
     void release() {
         if (p) PINNED ? cudaFreeHost(p) : cudaFree(p);
@@ -53,13 +59,23 @@ struct Layout {
     size_t add(size_t bytes) { const size_t off = (total + 255) & ~(size_t)255; total = off + bytes; return off; }
 };
 
-// a CUDA event destroyed with its owner
+// A CUDA event, and a CUDA stream (the library's own are non-blocking).  create() makes the handle on its first call only, so a
+// member created on first use is created once however often that use is reached, also after a failed attempt.
 struct Event {
     cudaEvent_t e = nullptr;
     Event() = default;
     Event(const Event&) = delete;
     Event& operator=(const Event&) = delete;
     ~Event() { if (e) cudaEventDestroy(e); }
+    cudaError_t create(unsigned flags) { return e ? cudaSuccess : cudaEventCreateWithFlags(&e, flags); }
+};
+struct Stream {
+    cudaStream_t s = nullptr;
+    Stream() = default;
+    Stream(const Stream&) = delete;
+    Stream& operator=(const Stream&) = delete;
+    ~Stream() { if (s) cudaStreamDestroy(s); }
+    cudaError_t create(unsigned flags) { return s ? cudaSuccess : cudaStreamCreateWithFlags(&s, flags); }
 };
 
 // 128-bit vector access: an fe is two uint4, an affine point four, an XYZZ point eight.

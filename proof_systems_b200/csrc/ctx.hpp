@@ -70,26 +70,28 @@ struct zk_ctx {
     // ordered) and handle-bound calls stay on the primary lane.  A caller-provided stream (zk_ctx_set_stream) or profiling mode
     // pins everything to the primary lane.  Resident bases and twiddle tables are shared, read-only.
     zk_ctx* parent = nullptr;                  // children point at the primary lane
-    std::vector<zk_ctx*> children;
+    std::vector<std::unique_ptr<zk_ctx>> children;
     int n_lanes = 4;                           // zk_ctx_set_option("ctx_lanes")
     unsigned rr = 0;                           // round-robin start of the next acquisition (guarded by pool_mu)
     std::mutex pool_mu;                        // children list
     std::mutex tab_mu;                         // NTT table cache of the primary lane (shared by all lanes)
     int device = 0;
     int sm_count = 132;                        // SMs of the device (the MSM sizes its grids by them)
-    cudaStream_t own_stream = nullptr, stream = nullptr;
+    zkb::Stream own_stream;
+    cudaStream_t stream = nullptr;       // own_stream, or the caller's (zk_ctx_set_stream)
     std::mutex mu;                       // a context serialises its calls (SRS: Sync + Send, SURVEY.md §8b "Threading")
     zkb::MsmWorkspace ws;                // scratch of the MSM pipeline (runs on `stream`)
     static constexpr int SIDE_STREAMS = 2;   // copy-in / copy-out streams of the pipelined host-pointer NTT (zk_ntt_batch)
-    cudaStream_t side[SIDE_STREAMS] = {};
+    zkb::Stream side[SIDE_STREAMS];
     zkb::MsmTuning msm;                  // zk_ctx_set_option("msm_batch", "msm_chunk", "msm_wave_threads")
-    cudaEvent_t ev_fork = nullptr;
-    cudaEvent_t ev_switch = nullptr;     // zk_ctx_set_stream: the new stream waits for the old one
+    zkb::Event ev_fork;
+    zkb::Event ev_switch;                // zk_ctx_set_stream: the new stream waits for the old one
     zkb::DevScratch d_scalars;           // staging for host-pointer MSM calls
     zkb::DevScratch d_ntt;               // staging for host-pointer NTT calls
     zkb::DevScratch d_ntt_tmp;           // second buffer of the two-pass plan
-    zkb::fe* ntt_small[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};  // [field][inverse] w_1024^(+-i)
-    std::map<unsigned, zkb::NttTables> ntt_tables;                         // key: field | inverse << 1 | log_n << 2
+    // NTT table cache of the primary lane: an entry exists only once its build has succeeded
+    zkb::DevScratch ntt_small[2][2];                   // [field][inverse] w_1024^(+-i), 512 entries
+    std::map<unsigned, zkb::NttTables> ntt_tables;     // key: field | inverse << 1 | log_n << 2
     zkb::DevScratch d_gather_sum;        // zk_msm_finish_gathered: cross-rank sums of the slice sums
     zkb::PinnedScratch h_gather;         // ... and their pinned host copy
     zkb::PinnedScratch h_pinned_slots;   // zkb::PinnedSlots, through ctx_pinned
@@ -104,12 +106,20 @@ struct zk_ctx {
     uint64_t launches = 0;
     bool profile = false;                // per-stage device timing (zk_ctx_set_profile)
     std::atomic<bool> pinned{false};     // host-pointer calls stay on the primary lane (stream, profile, n_lanes; written under mu)
-    cudaEvent_t ev_ntt[2] = {nullptr, nullptr};
+    zkb::Event ev_ntt[2];
     float ntt_ms = 0;                    // device time of the last profiled NTT call (all its kernels)
-    // frees the scratch members; hidden like the library's other C++ symbols (zkb200.h gives the type default visibility)
-    __attribute__((visibility("hidden"))) ~zk_ctx() = default;
+    // The child lanes go first (their work reads this lane's tables), then the lane waits for its streams; the members then free
+    // themselves on the device zk_ctx_destroy made current.  Hidden like the library's other C++ symbols (zkb200.h gives the type
+    // default visibility).
+    __attribute__((visibility("hidden"))) ~zk_ctx() {
+        children.clear();
+        if (stream) cudaStreamSynchronize(stream);
+        for (auto& s : side)
+            if (s.s) cudaStreamSynchronize(s.s);
+    }
 };
 
+// freed by zk_bases_free, which takes the context lock and makes its device current
 struct zk_bases {
     zk_ctx* ctx = nullptr;
     zkb::MsmBases b;

@@ -71,10 +71,11 @@ template <class F, class FS> int lagrange_basis_build(const MsmBases& g, unsigne
     const size_t start = (size_t)chunk * g.n;
     if (start >= n && !(chunk == 0 && n <= g.n)) { zk_set_error("lagrange_basis: chunk %u outside a domain of %u over %zu generators", chunk, n, g.n); return ZK_ERR_INVALID; }
     const unsigned terms = (unsigned)std::min<size_t>(g.n, n - start);
-    xyzz_t* a = nullptr;
-    fe* tw = nullptr;
-    ZK_CUDA(cudaMalloc(&a, (size_t)n * sizeof(xyzz_t)));
-    ZK_CUDA(cudaMalloc(&tw, ((size_t)n / 2 + 2) * sizeof(fe)));
+    DevScratch a_mem, tw_mem;
+    if (int rc = a_mem.ensure((size_t)n * sizeof(xyzz_t))) return rc;
+    if (int rc = tw_mem.ensure(((size_t)n / 2 + 2) * sizeof(fe))) return rc;
+    xyzz_t* a = a_mem.at<xyzz_t>();
+    fe* tw = tw_mem.at<fe>();
     fe* ninv = tw + n / 2 + 1;
     const unsigned ntw = n / 2 ? n / 2 : 1;
     k_gntt_twiddles<FS><<<(ntw + 127) / 128, 128, 0, st>>>(tw, ninv, log_n, ntw);
@@ -83,8 +84,6 @@ template <class F, class FS> int lagrange_basis_build(const MsmBases& g, unsigne
     k_gntt_finish<F><<<(n + 127) / 128, 128, 0, st>>>(a, ninv, d_out, log_n);
     cudaError_t e = cudaGetLastError();
     cudaError_t e2 = cudaStreamSynchronize(st);
-    cudaFree(a);
-    cudaFree(tw);
     if (e != cudaSuccess || e2 != cudaSuccess) { zk_set_error("lagrange_basis: %s", cudaGetErrorString(e != cudaSuccess ? e : e2)); return ZK_ERR_CUDA; }
     if (launches) *launches += 3 + log_n;
     return ZK_OK;

@@ -50,7 +50,7 @@ struct zk_index_cache {
     zk_index_header hdr{};
     struct Section { uint32_t tag; uint64_t offset, length; uint32_t elem_domain_size; };
     std::vector<Section> sections;
-    uint8_t* d_payload = nullptr;     // image bytes [lo, hi) as they lie in the file
+    zkb::DevScratch payload;          // image bytes [lo, hi) as they lie in the file
     uint64_t lo = 0, hi = 0;
 };
 
@@ -78,7 +78,7 @@ int zk_index_cache_load(zk_ctx* ctx, const void* image, size_t image_len, const 
     }
     const uint32_t num_sections = rd32(id + IDENTIFIER_MAX_LEN);
     const uint8_t* h = p + PREAMBLE_SIZE;
-    zk_index_cache* c = new zk_index_cache();
+    auto c = std::make_unique<zk_index_cache>();
     c->ctx = ctx;
     zk_index_header& H = c->hdr;
     H.public_inputs = rd32(h); H.prev_challenges = rd32(h + 4); H.zk_rows = rd64(h + 8); H.max_poly_size = rd64(h + 16);
@@ -94,23 +94,23 @@ int zk_index_cache_load(zk_ctx* ctx, const void* image, size_t image_len, const 
     H.identifier[id_len < IDENTIFIER_MAX_LEN ? id_len : IDENTIFIER_MAX_LEN - 1] = 0;
     if (H.domain_d1_size == 0 || (H.domain_d1_size & (H.domain_d1_size - 1)) || H.domain_d1_size > ((uint64_t)1 << 29)) {
         zk_set_error("index_cache: stored d1 domain size %llu is not a valid evaluation domain", (unsigned long long)H.domain_d1_size);
-        delete c; return ZK_ERR_INVALID;
+        return ZK_ERR_INVALID;
     }
     const size_t table_off = PREAMBLE_SIZE + SCALAR_HEADER_SIZE;
-    if (image_len < table_off + (size_t)num_sections * SECTION_ENTRY_SIZE) { zk_set_error("index_cache: cache file truncated before end of declared payload"); delete c; return ZK_ERR_INVALID; }
+    if (image_len < table_off + (size_t)num_sections * SECTION_ENTRY_SIZE) { zk_set_error("index_cache: cache file truncated before end of declared payload"); return ZK_ERR_INVALID; }
     uint64_t lo = UINT64_MAX, hi = 0;
     for (uint32_t s = 0; s < num_sections; s++) {
         const uint8_t* e = p + table_off + (size_t)s * SECTION_ENTRY_SIZE;
         zk_index_cache::Section sec{rd32(e), rd64(e + 4), rd64(e + 12), rd32(e + 20)};
         for (const auto& o : c->sections)
-            if (o.tag == sec.tag) { zk_set_error("index_cache: duplicate section tag %#x in section table", sec.tag); delete c; return ZK_ERR_INVALID; }
-        if (sec.offset % 32) { zk_set_error("index_cache: section %#x offset %llu is not 32-byte aligned", sec.tag, (unsigned long long)sec.offset); delete c; return ZK_ERR_INVALID; }
-        if (sec.offset > image_len || sec.length > image_len - sec.offset) { zk_set_error("index_cache: cache file truncated before end of declared payload"); delete c; return ZK_ERR_INVALID; }
+            if (o.tag == sec.tag) { zk_set_error("index_cache: duplicate section tag %#x in section table", sec.tag); return ZK_ERR_INVALID; }
+        if (sec.offset % 32) { zk_set_error("index_cache: section %#x offset %llu is not 32-byte aligned", sec.tag, (unsigned long long)sec.offset); return ZK_ERR_INVALID; }
+        if (sec.offset > image_len || sec.length > image_len - sec.offset) { zk_set_error("index_cache: cache file truncated before end of declared payload"); return ZK_ERR_INVALID; }
         if (is_field_section(sec.tag)) {
-            if (sec.length % 32) { zk_set_error("index_cache: section %#x payload length %llu is not a multiple of 32", sec.tag, (unsigned long long)sec.length); delete c; return ZK_ERR_INVALID; }
+            if (sec.length % 32) { zk_set_error("index_cache: section %#x payload length %llu is not a multiple of 32", sec.tag, (unsigned long long)sec.length); return ZK_ERR_INVALID; }
             if (sec.elem_domain_size && sec.tag != 0x50 && sec.length != (uint64_t)sec.elem_domain_size * 32) {
                 zk_set_error("index_cache: section %#x length mismatch: expected %llu, found %llu", sec.tag, (unsigned long long)sec.elem_domain_size * 32, (unsigned long long)sec.length);
-                delete c; return ZK_ERR_INVALID;
+                return ZK_ERR_INVALID;
             }
             if (sec.length) { lo = std::min(lo, sec.offset); hi = std::max(hi, sec.offset + sec.length); }
         }
@@ -120,30 +120,27 @@ int zk_index_cache_load(zk_ctx* ctx, const void* image, size_t image_len, const 
     for (uint32_t tag : {0x30u, 0x31u, 0x32u, 0x33u, 0x34u, 0x35u, 0x36u}) {
         bool found = false;
         for (const auto& o : c->sections) found |= o.tag == tag;
-        if (!found) { zk_set_error("index_cache: required section tag %#x missing from section table", tag); delete c; return ZK_ERR_INVALID; }
+        if (!found) { zk_set_error("index_cache: required section tag %#x missing from section table", tag); return ZK_ERR_INVALID; }
     }
     std::lock_guard<std::mutex> lk(ctx->mu);
     ZK_CUDA(cudaSetDevice(ctx->device));
     if (hi > lo) {
         c->lo = lo; c->hi = hi;
-        cudaError_t e = cudaMalloc(&c->d_payload, hi - lo);
+        if (int rc = c->payload.ensure(hi - lo)) return rc;
         // ONE copy of the payload as it lies in the mapping: the bytes are already the device's field-element format
-        if (e == cudaSuccess) e = cudaMemcpyAsync(c->d_payload, p + lo, hi - lo, cudaMemcpyHostToDevice, ctx->stream);
+        cudaError_t e = cudaMemcpyAsync(c->payload.p, p + lo, hi - lo, cudaMemcpyHostToDevice, ctx->stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-        if (e != cudaSuccess) { zk_set_error("index_cache: %s", cudaGetErrorString(e)); if (c->d_payload) cudaFree(c->d_payload); delete c; return ZK_ERR_CUDA; }
+        if (e != cudaSuccess) { zk_set_error("index_cache: %s", cudaGetErrorString(e)); return ZK_ERR_CUDA; }
     }
-    *out = c;
+    *out = c.release();
     return ZK_OK;
 }
 
 void zk_index_cache_free(zk_index_cache* c) {
     if (!c) return;
-    {
-        std::lock_guard<std::mutex> lk(c->ctx->mu);
-        cudaSetDevice(c->ctx->device);
-        cudaStreamSynchronize(c->ctx->stream);
-        if (c->d_payload) cudaFree(c->d_payload);
-    }
+    std::lock_guard<std::mutex> lk(c->ctx->mu);
+    cudaSetDevice(c->ctx->device);
+    cudaStreamSynchronize(c->ctx->stream);
     delete c;
 }
 
@@ -160,7 +157,7 @@ int zk_index_cache_section(const zk_index_cache* c, uint32_t tag, const void** d
     for (const auto& s : c->sections) {
         if (s.tag != tag) continue;
         if (!is_field_section(tag)) { zk_set_error("index_cache_section: section %#x does not hold field elements", tag); return ZK_ERR_INVALID; }
-        *d_ptr = s.length ? c->d_payload + (s.offset - c->lo) : nullptr;
+        *d_ptr = s.length ? c->payload.at<uint8_t>(s.offset - c->lo) : nullptr;
         *n_elems = s.length / 32;
         if (elem_domain_size) *elem_domain_size = s.elem_domain_size;
         return ZK_OK;

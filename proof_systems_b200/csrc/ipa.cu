@@ -117,12 +117,6 @@ template <class FS> static int ipa_expand_and_msm(zk_ipa* s, size_t h, uint64_t 
     return ZK_OK;
 }
 
-void ipa_release(zk_ipa* s) {
-    if (!s) return;
-    if (s->owns_storage) cudaFree(s->d_a);
-    delete s;
-}
-
 // one device allocation: a | b | s0 | s1 | sc_L (+2) | sc_R (+2) | partials (+ two inner products)
 size_t ipa_storage_bytes(size_t n) { return (6 * n + 4 + IP_BLOCKS + 2) * sizeof(fe); }
 
@@ -131,24 +125,22 @@ int ipa_create(zk_ctx* ctx, const zk_bases* bases, size_t n, zk_ipa** out, void*
     if (bases->b.n > n || (n > 1 && 2 * bases->b.n <= n)) { zk_set_error("ipa: n = %zu is not the SRS size %zu rounded up to a power of two", n, bases->b.n); return ZK_ERR_INVALID; }
     PinnedSlots* pin = ctx_pinned(ctx);
     if (!pin) return ZK_ERR_CUDA;
-    zk_ipa* s = new zk_ipa();
+    auto s = std::make_unique<zk_ipa>();
     s->ctx = ctx; s->curve = bases->b.curve; s->n = s->n0 = n; s->bases = bases;
-    cudaError_t e = cudaSuccess;
-    if (storage) { s->d_a = (fe*)storage; s->owns_storage = false; }
-    else e = cudaMalloc(&s->d_a, ipa_storage_bytes(n));
-    if (e == cudaSuccess) {
-        s->d_b = s->d_a + n; s->d_s[0] = s->d_a + 2 * n; s->d_s[1] = s->d_a + 3 * n; s->d_sc = s->d_a + 4 * n; s->d_part = s->d_a + 6 * n + 4;
-        s->h_ip = pin->ip;
-        // s_0 = (1), staged through the curve's slot (PinnedSlots::s0)
-        const fe* one = with_curve(s->curve, [&](auto c) { using C = decltype(c); return &(pin->s0[C::scalar_field] = fe_one<typename C::FS>()); });
-        e = cudaMemcpyAsync(s->d_s[0], one, sizeof(fe), cudaMemcpyHostToDevice, ctx->stream);
+    if (!storage) {
+        if (int rc = s->storage.ensure(ipa_storage_bytes(n))) return rc;
+        storage = s->storage.p;
     }
-    if (e != cudaSuccess) {
+    s->d_a = (fe*)storage;
+    s->d_b = s->d_a + n; s->d_s[0] = s->d_a + 2 * n; s->d_s[1] = s->d_a + 3 * n; s->d_sc = s->d_a + 4 * n; s->d_part = s->d_a + 6 * n + 4;
+    s->h_ip = pin->ip;
+    // s_0 = (1), staged through the curve's slot (PinnedSlots::s0)
+    const fe* one = with_curve(s->curve, [&](auto c) { using C = decltype(c); return &(pin->s0[C::scalar_field] = fe_one<typename C::FS>()); });
+    if (cudaError_t e = cudaMemcpyAsync(s->d_s[0], one, sizeof(fe), cudaMemcpyHostToDevice, ctx->stream)) {
         zk_set_error("ipa: %s", cudaGetErrorString(e));
-        ipa_release(s);
         return ZK_ERR_CUDA;
     }
-    *out = s;
+    *out = s.release();
     return ZK_OK;
 }
 
@@ -219,15 +211,15 @@ int zk_ipa_begin(zk_ctx* ctx, const zk_bases* bases, const uint64_t* a_mont, con
     zk_ipa* s = nullptr;
     int rc = ipa_create(ctx, bases, n, &s);
     if (rc) return rc;
+    std::unique_ptr<zk_ipa> owner(s);
     cudaError_t e = cudaMemcpyAsync(s->d_a, a_mont, n * sizeof(fe), cudaMemcpyHostToDevice, ctx->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(s->d_b, b_mont, n * sizeof(fe), cudaMemcpyHostToDevice, ctx->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
     if (e != cudaSuccess) {
         zk_set_error("ipa_begin: %s", cudaGetErrorString(e));
-        ipa_release(s);
         return ZK_ERR_CUDA;
     }
-    *out = s;
+    *out = owner.release();
     return ZK_OK;
 }
 
@@ -235,7 +227,7 @@ void zk_ipa_free(zk_ipa* s) {
     if (!s) return;
     std::lock_guard<std::mutex> lk(s->ctx->mu);
     cudaSetDevice(s->ctx->device);
-    ipa_release(s);
+    delete s;
 }
 
 size_t zk_ipa_len(const zk_ipa* s) { return s ? s->n : 0; }

@@ -69,7 +69,8 @@ template <class F> int msm_bases_create(MsmBases& b, const affine_t* pts, bool p
     b.c = c_table;
     b.nwin = c_table ? msm_num_windows(c_table) : 0;
     size_t rows = c_table ? b.nwin : 1;
-    ZK_CUDA(cudaMalloc(&b.d_points, std::max<size_t>(rows * n, 1) * sizeof(affine_t)));
+    if (int rc = b.points.ensure(std::max<size_t>(rows * n, 1) * sizeof(affine_t))) return rc;
+    b.d_points = b.points.at<affine_t>();
     if (n == 0) return ZK_OK;
     ZK_CUDA(cudaMemcpyAsync(b.d_points, pts, n * sizeof(affine_t), pts_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
     if (c_table) {
@@ -79,11 +80,6 @@ template <class F> int msm_bases_create(MsmBases& b, const affine_t* pts, bool p
     }
     ZK_CUDA(cudaStreamSynchronize(st));
     return ZK_OK;
-}
-
-void msm_bases_free(MsmBases& b) {
-    if (b.d_points) cudaFree(b.d_points);
-    b = MsmBases();
 }
 
 // ---------------------------------------------------------------------------------------------- recode + histogram
@@ -589,8 +585,8 @@ int msm_run(const MsmBases& b, const size_t* offs, size_t n_main, const fe* cons
     uint32_t *d_meta = ws.fixed.at<uint32_t>(o_meta), *d_giants = ws.fixed.at<uint32_t>(o_giants), *d_giant_tickets = ws.fixed.at<uint32_t>(o_tickets);
     xyzz_t* d_giant_slices = ws.fixed.at<xyzz_t>(o_slices);
     unsigned nl = 0;
-    if (profile && !ws.ev[0].e)
-        for (int s = 0; s <= MSM_ST_COUNT; s++) ZK_CUDA(cudaEventCreate(&ws.ev[s].e));
+    if (profile)
+        for (Event& ev : ws.ev) ZK_CUDA(ev.create(cudaEventDefault));
 #define STAGE_MARK(s) do { if (profile) ZK_CUDA(cudaEventRecord(ws.ev[s].e, st)); } while (0)
 
     MsmScalarSet sc{};

@@ -45,7 +45,8 @@ struct MsmBases {
     size_t n = 0;              // number of points
     unsigned c = 0;            // window bits of the precomputed table (0: no table)
     unsigned nwin = 0;         // windows in the table
-    affine_t* d_points = nullptr;  // [max(1,nwin)][n]  row w holds 2^(c*w) * P_i
+    affine_t* d_points = nullptr;  // [max(1,nwin)][n]  row w holds 2^(c*w) * P_i: in `points`, or a view (zk_srs_verify's proof points)
+    DevScratch points;
 };
 
 // Per-stage device timing of a profiled run (CUDA events on the launching stream).
@@ -81,7 +82,6 @@ unsigned msm_num_windows(unsigned c);
 
 // Upload n affine points (host or device memory, 16 u32 each) and optionally build the window table.
 template <class F> int msm_bases_create(MsmBases& b, const affine_t* pts, bool pts_on_device, size_t n, unsigned c_table, cudaStream_t st);
-void msm_bases_free(MsmBases& b);
 
 // What msm_run leaves in ws.h_bitsums (or at d_out): k x groups x c XYZZ points T[j][g][t]; MSM j is sum_g 2^(c g) sum_t 2^t T[j][g][t].
 struct MsmResultShape {

@@ -56,21 +56,22 @@ template <class F> __global__ void k_full_table(fe* full, const fe* __restrict__
 }
 
 template <class F> int ntt_build_small_table(fe* d_small, bool inverse, cudaStream_t st) {
-    fe* bases;
-    ZK_CUDA(cudaMalloc(&bases, 8 * sizeof(fe)));
+    DevScratch tmp;
+    if (int rc = tmp.ensure(8 * sizeof(fe))) return rc;
+    fe* bases = tmp.at<fe>();
     k_ntt_setup<F><<<1, 32, 0, st>>>(bases, 10, inverse ? 1 : 0);
     k_pow_table<F><<<2, 256, 0, st>>>(d_small, bases + 0, bases + 5, 512);
     ZK_CUDA(cudaGetLastError());
     ZK_CUDA(cudaStreamSynchronize(st));
-    ZK_CUDA(cudaFree(bases));
     return ZK_OK;
 }
 
 template <class F> int ntt_build_tables(NttTables& t, unsigned log_n, bool inverse, cudaStream_t st) {
-    fe* bases;
-    ZK_CUDA(cudaMalloc(&bases, 8 * sizeof(fe)));
-    fe* blk;
-    ZK_CUDA(cudaMalloc(&blk, 6 * 1024 * sizeof(fe)));
+    DevScratch tmp;
+    if (int rc = tmp.ensure(8 * sizeof(fe))) return rc;
+    fe* bases = tmp.at<fe>();
+    if (int rc = t.block.ensure(6 * 1024 * sizeof(fe))) return rc;
+    fe* blk = t.block.at<fe>();
     t.lo = blk; t.ulo = blk + 1024; t.mid = blk + 2048; t.hi2 = blk + 3072; t.clo = blk + 4096; t.chi = blk + 5120;
     k_ntt_setup<F><<<1, 32, 0, st>>>(bases, log_n, inverse ? 1 : 0);
     k_pow_table<F><<<4, 256, 0, st>>>(t.lo, bases + 0, bases + 4, 1024);   // w^i * (n^-1 if inverse)
@@ -79,23 +80,15 @@ template <class F> int ntt_build_tables(NttTables& t, unsigned log_n, bool inver
     k_pow_table<F><<<4, 256, 0, st>>>(t.hi2, bases + 6, bases + 5, 1024);  // w^(2^20 i)
     k_pow_table<F><<<4, 256, 0, st>>>(t.clo, bases + 2, bases + 5, 1024);  // g^i
     k_pow_table<F><<<4, 256, 0, st>>>(t.chi, bases + 3, bases + 5, 1024);  // g^(1024 i)
-    t.full = nullptr;
     if (log_n > NTT_MAX_LOG_SUB && log_n <= 2 * NTT_MAX_LOG_SUB) {     // only the two-pass plan reads it (ntt_run)
         const size_t n = (size_t)1 << log_n;
         const unsigned log_n1 = (log_n + 1) / 2;
-        ZK_CUDA(cudaMalloc(&t.full, n * sizeof(fe)));
-        k_full_table<F><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(t.full, t.lo, t.mid, log_n1, n);
+        if (int rc = t.full.ensure(n * sizeof(fe))) return rc;
+        k_full_table<F><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(t.full.at<fe>(), t.lo, t.mid, log_n1, n);
     }
     ZK_CUDA(cudaGetLastError());
     ZK_CUDA(cudaStreamSynchronize(st));
-    ZK_CUDA(cudaFree(bases));
     return ZK_OK;
-}
-
-void ntt_free_tables(NttTables& t) {
-    if (t.lo) cudaFree(t.lo);
-    if (t.full) cudaFree(t.full);
-    t = NttTables();
 }
 
 // ---------------------------------------------------------------------------------------------- the tile pass
@@ -301,8 +294,8 @@ int ntt_run(const fe* d_in, size_t in_bs, fe* d_out, fe* d_tmp, const fe* d_smal
         // pass 1: n2 column transforms of size n1 (stride n2), times w_n^(j2 k1); in -> tmp, layout [k1][j2]
         NttPassParams p{};
         p.in = d_in; p.out = d_tmp; p.small = d_small;
-        p.tw_full = tabs.full;
-        if (!tabs.full) { p.lo = tabs.lo; p.mid = tabs.mid; p.hi2 = tabs.hi2; }
+        p.tw_full = tabs.full.at<fe>();
+        if (!tabs.full.p) { p.lo = tabs.lo; p.mid = tabs.mid; p.hi2 = tabs.hi2; }
         p.log_s = log_n1; p.split_log = 0;
         p.in_hi = 1; p.in_rs = n2; p.in_bs = in_bs;
         p.out_hi = 1; p.out_rs = n2; p.out_bs = n;

@@ -26,15 +26,16 @@ namespace zkb {
 constexpr unsigned NTT_MAX_LOG_SUB = 10;   // sub-transform size limit (one column per tile, twiddles from a 512-entry table)
 constexpr unsigned NTT_MAX_LOG_N = 30;     // three passes of <= 2^10
 
-// device tables of one (field, log_n, direction)
+// device tables of one (field, log_n, direction), owned: lo .. chi are views into `block`
 struct NttTables {
+    DevScratch block;
     fe* lo = nullptr;    // [1024] w_n^(+-i)            (inverse: times n^-1)
     fe* ulo = nullptr;   // [1024] w_n^(+-i)            unscaled (the middle pass of a three-pass plan uses the tables of n2 * n3)
     fe* mid = nullptr;   // [1024] w_n^(+-1024 i)
     fe* hi2 = nullptr;   // [1024] w_n^(+-2^20 i)
     fe* clo = nullptr;   // [1024] g^(+-i)              coset powers
     fe* chi = nullptr;   // [1024] g^(+-1024 i)
-    fe* full = nullptr;  // [n]    w_n^(+-(col * k)) (inverse: times n^-1) at index col * n1 + k: contiguous per tile of pass 1; null outside 2^10 < n <= 2^20
+    DevScratch full;     // [n]    w_n^(+-(col * k)) (inverse: times n^-1) at index col * n1 + k: contiguous per tile of pass 1; empty outside 2^10 < n <= 2^20
 };
 
 // One pass = independent S-point transforms of columns ("tiles").  Tile tau = (t_hi << split_log) | t_lo of polynomial b reads
@@ -60,7 +61,6 @@ struct NttPassParams {
 
 template <class F> int ntt_build_small_table(fe* d_small, bool inverse, cudaStream_t st);
 template <class F> int ntt_build_tables(NttTables& t, unsigned log_n, bool inverse, cudaStream_t st);
-void ntt_free_tables(NttTables& t);
 // log2(n2 * n3) of the three-pass plan for a transform of 2^log_n elements (0: one or two passes, no inner tables needed)
 unsigned ntt_inner_log(unsigned log_n);
 

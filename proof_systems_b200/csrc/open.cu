@@ -182,7 +182,7 @@ static int open_impl(zk_srs* srs, const zk_open_poly* polys, size_t n_polys, con
     if (rc) return rc;
     rc = ipa_create(ctx, srs->g, n0, &s, ctx->d_ipa.p);
     if (rc) return rc;
-    struct Guard { zk_ipa* s; ~Guard() { cudaStreamSynchronize(s->ctx->stream); ipa_release(s); } } guard{s};
+    struct Guard { zk_ipa* s; ~Guard() { cudaStreamSynchronize(s->ctx->stream); delete s; } } guard{s};
     std::vector<CombineDesc> all_terms(coeff_terms);
     all_terms.insert(all_terms.end(), eval_terms.begin(), eval_terms.end());
     if (!all_terms.empty()) ZK_CUDA(cudaMemcpyAsync(d_descs, all_terms.data(), all_terms.size() * sizeof(CombineDesc), cudaMemcpyHostToDevice, st));
