@@ -100,6 +100,43 @@ pub struct zk_dev_poly {
     pub len: u64,
 }
 
+/// zk_lookup_term: coeff (Montgomery) * w[column][row + next]
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct zk_lookup_term {
+    pub coeff: [u64; 4],
+    pub column: u32,
+    pub next: u32,
+}
+
+/// zk_lookup_joint: one JointLookupSpec; entry e is entry_terms[e] consecutive terms from first_term on
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct zk_lookup_joint {
+    pub table_id: i32,
+    pub table_id_column: i32, // -1: Constant(table_id), else WitnessColumn
+    pub n_entries: u32,
+    pub entry_terms: [u32; 4],
+    pub first_term: u32,
+}
+
+/// zk_lookup_info: LookupInfo lowered (patterns of lookups, each row's pattern: 0 none, p + 1 pattern p)
+#[repr(C)]
+pub struct zk_lookup_info {
+    pub terms: *const zk_lookup_term,
+    pub n_terms: usize,
+    pub lookups: *const zk_lookup_joint,
+    pub n_lookups: usize,
+    pub pattern_first: *const u32,
+    pub pattern_count: *const u32,
+    pub n_patterns: usize,
+    pub row_pattern: *const u8,
+    pub max_per_row: c_uint,
+    pub joint_combiner: [u64; 4],
+    pub table_id_combiner: [u64; 4],
+    pub dummy: [u64; 4],
+}
+
 #[repr(C)]
 #[derive(Copy, Clone)]
 pub struct zk_lin_term {
@@ -158,6 +195,15 @@ extern "C" {
     pub fn zk_prover_ft_dev(ctx: *mut zk_ctx, field_id: c_int, log_n: c_uint, max_poly_size: usize, terms: *const zk_lin_term, n_terms: usize,
                             d_t: *const c_void, t_len: usize, zeta_mont: *const u64, d_ft: *mut c_void, ft_len: *mut usize,
                             ft_eval1: *mut u64) -> c_int;
+    pub fn zk_lookup_joint_table_dev(ctx: *mut zk_ctx, field_id: c_int, log_n: c_uint, d_cols: *const *const c_void, n_cols: usize,
+                                     d_table_ids8: *const c_void, d_runtime8: *const c_void, joint_combiner: *const u64,
+                                     table_id_combiner: *const u64, d_out8: *mut c_void, d_out1: *mut c_void) -> c_int;
+    pub fn zk_lookup_sorted_dev(ctx: *mut zk_ctx, field_id: c_int, log_n: c_uint, zk_rows: usize, d_w: *const *const c_void,
+                                d_table: *const c_void, table_stride: c_uint, info: *const zk_lookup_info, rand: *const u64,
+                                d_sorted: *const *mut c_void, not_in_table_row: *mut i64) -> c_int;
+    pub fn zk_lookup_aggreg_dev(ctx: *mut zk_ctx, field_id: c_int, log_n: c_uint, zk_rows: usize, d_w: *const *const c_void,
+                                d_table: *const c_void, table_stride: c_uint, info: *const zk_lookup_info, d_sorted: *const *const c_void,
+                                beta: *const u64, gamma: *const u64, rand: *const u64, d_aggreg: *mut c_void, final_is_one: *mut c_int) -> c_int;
     pub fn zk_perm_aggreg_dev(ctx: *mut zk_ctx, field_id: c_int, log_n: c_uint, zk_rows: usize, d_w: *const *const c_void,
                               d_sigma: *const *const c_void, sigma_len: u64, beta: *const u64, gamma: *const u64, shifts: *const u64,
                               rand: *const u64, d_z: *mut c_void, final_is_one: *mut c_int) -> c_int;

@@ -15,6 +15,8 @@
 //!   and sigma_6 over d8, leaving ft resident for the opening proof (`zk_prover_ft_dev`).
 //! * [`perm::perm_aggreg_dev`] builds the permutation aggregation polynomial z (kimchi/src/circuits/polynomials/permutation.rs:447-574)
 //!   from the resident witness and `permutation_coefficients8`, leaving z resident (`zk_perm_aggreg_dev`).
+//! * [`lookup::LookupLowering`] builds the lookup argument's joint table, sorted columns and aggregation polynomial
+//!   (kimchi/src/prover.rs:383-673) from the resident witness and the index cache's lookup tables (`zk_lookup_*_dev`).
 //!
 //! Everything called is declared in include/zkb200.h and exported by libzkb200.so; there is no CPU fallback inside the library
 //! (`Ctx::new` fails without a CUDA device) — code that must also run without a GPU keeps using `ipa::SRS`.
@@ -23,6 +25,7 @@ pub mod evals;
 pub mod expr;
 pub mod ffi;
 pub mod ft;
+pub mod lookup;
 pub mod marshal;
 pub mod open;
 pub mod perm;

@@ -348,6 +348,71 @@ int zk_perm_aggreg_dev(zk_ctx* ctx, int field_id, unsigned log_n, size_t zk_rows
                        uint64_t sigma_len, const uint64_t beta[4], const uint64_t gamma[4], const uint64_t shifts[28], const uint64_t rand[8],
                        void* d_z, int* final_is_one);
 
+/* ------------------------------------------------------------------ lookup argument (kimchi/src/prover.rs:383-673)
+ * The joint lookup table, the sorted columns and the lookup aggregation polynomial over resident operands.  With n = 2^log_n,
+ * L = n - zk_rows - 1 (lookup_rows), m = max_per_row, jc = joint_combiner, tic = table_id_combiner:
+ *
+ * zk_lookup_joint_table_dev   T8[i] = sum_c jc^c col_c[i] + tic tid8[i] at every point of d8 (combine_table_entry,
+ *                             lookup/tables/mod.rs:167-182; prover.rs:500-568).  d_cols: n_cols (1 .. 16) columns of 8n evaluations
+ *                             (a cached index's section 0x50); d_table_ids8: NULL (table id 0) or 8n evaluations (section 0x51);
+ *                             d_runtime8: NULL or the runtime table contribution over d8, added to column 1 (n_cols >= 2).
+ *                             d_out8 receives 8n evaluations, d_out1 (NULL or n elements) the d1 values T1[i] = T8[8 i].
+ *                             Returns with its work queued on the context's stream.
+ * zk_lookup_sorted_dev        lookup::constraints::sorted then zk_patch (constraints.rs:35-48, 90-201): the m + 1 snake-shaped
+ *                             sorted columns of the witness's joint lookup values and T1[0 .. L), rows L + 1 .. n - 1 of column k
+ *                             = rand[k zk_rows .. (k + 1) zk_rows) (the reference's draws, column by column).  A lookup value
+ *                             missing from T1[0 .. L) sets *not_in_table_row to the smallest such row
+ *                             (ProverError::ValueNotInTable) and leaves d_sorted untouched; otherwise it is -1.
+ * zk_lookup_aggreg_dev        lookup::constraints::aggregation (constraints.rs:233-338): agg[0] = 1,
+ *                             agg[i + 1] = agg[i] f_i t_i / den_i for i < L (a zero den_i inverts to zero), rows L + 1 .. n - 1 =
+ *                             rand[0 .. zk_rows); *final_is_one = (agg[L] == 1), the reference's debug assertion.
+ * The table T1 is read as d_table[table_stride i] for i <= L (8: the joint table over d8, 1: over d1).  d_w: the 15 witness columns
+ * as n d1 evaluations each.  Outputs are d1 EVALUATIONS (what commit_evaluations takes; zk_ntt_dev_oop gives coefficients and d8).
+ *
+ * zk_lookup_info: the circuit's LookupInfo lowered once per index.  A joint lookup (JointLookupSpec) has n_entries <= 4 entries;
+ * entry e is the sum of entry_terms[e] consecutive terms from terms[first_term] on (entry 0's first), each term coeff *
+ * w[column][row + next] (next: 0 current row, 1 next row).  Its table id is Constant(table_id) (i32_to_field) when
+ * table_id_column = -1, else WitnessColumn(table_id_column) at the current row.  Pattern p is lookups[pattern_first[p] ..
+ * pattern_first[p] + pattern_count[p]); row_pattern (host memory, L entries) gives each row's pattern: 0 = none, p + 1 = pattern p
+ * (LookupInfo::by_row).  Scalars are Montgomery field elements.
+ *
+ * The sorted and aggregation calls run on the context's stream and synchronise once.  Errors, before anything runs (outputs
+ * untouched): ZK_ERR_INVALID for a null pointer, an unknown field, log_n > 30, zk_rows outside [1, n - 2], m outside 1 .. 8,
+ * (m + 1) L >= 2^32, a pattern with more than m lookups or outside lookups, more than 255 patterns, a lookup with more than 4
+ * entries or terms outside terms, a column >= 15, next > 1, a table_id_column outside -1 .. 14, a row_pattern value > n_patterns,
+ * a scalar that is not a canonical field element, a table stride outside 1 .. 8, an output overlapping an input or another output.
+ * zk_lookup_sorted_dev also returns ZK_ERR_INVALID, d_sorted untouched, when the columns cannot be formed: the dummy value is
+ * missing from T1[0 .. L) while some row is padded (the reference builds malformed columns or panics there). */
+typedef struct zk_lookup_term { uint64_t coeff[4]; uint32_t column; uint32_t next; } zk_lookup_term;
+typedef struct zk_lookup_joint {
+    int32_t table_id;
+    int32_t table_id_column;
+    uint32_t n_entries;
+    uint32_t entry_terms[4];
+    uint32_t first_term;
+} zk_lookup_joint;
+typedef struct zk_lookup_info {
+    const zk_lookup_term* terms;
+    size_t n_terms;
+    const zk_lookup_joint* lookups;
+    size_t n_lookups;
+    const uint32_t* pattern_first;
+    const uint32_t* pattern_count;
+    size_t n_patterns;
+    const uint8_t* row_pattern;
+    unsigned max_per_row;
+    uint64_t joint_combiner[4], table_id_combiner[4], dummy[4];
+} zk_lookup_info;
+int zk_lookup_joint_table_dev(zk_ctx* ctx, int field_id, unsigned log_n, const void* const* d_cols, size_t n_cols, const void* d_table_ids8,
+                              const void* d_runtime8, const uint64_t joint_combiner[4], const uint64_t table_id_combiner[4], void* d_out8,
+                              void* d_out1);
+int zk_lookup_sorted_dev(zk_ctx* ctx, int field_id, unsigned log_n, size_t zk_rows, const void* const d_w[15], const void* d_table,
+                         unsigned table_stride, const zk_lookup_info* info, const uint64_t* rand, void* const* d_sorted,
+                         int64_t* not_in_table_row);
+int zk_lookup_aggreg_dev(zk_ctx* ctx, int field_id, unsigned log_n, size_t zk_rows, const void* const d_w[15], const void* d_table,
+                         unsigned table_stride, const zk_lookup_info* info, const void* const* d_sorted, const uint64_t beta[4],
+                         const uint64_t gamma[4], const uint64_t* rand, void* d_aggreg, int* final_is_one);
+
 /* ------------------------------------------------------------------ constraint evaluator (kimchi's expression framework)
  * zk_expr_eval_dev replaces Expr::evaluations(&env) (kimchi/src/circuits/expr.rs:1938-2190; call sites kimchi/src/prover.rs:794-892:
  * every gate's combined constraint and the lookup constraints, evaluated over d4 or d8 and added into t4 / t8).  The expression is

@@ -17,5 +17,5 @@ from ._lib import (  # noqa: F401
     jacobian_to_affine, jacobian_sum,
 )
 from .host import (  # noqa: F401
-    SRS, BatchEvaluationProof, ExprProgram, IndexCache, IpaRounds, LagrangeBasisEvaluations, OpeningProof, PolyComm, Radix2EvaluationDomain, srs_open, srs_verify,
+    SRS, BatchEvaluationProof, ExprProgram, IndexCache, IpaRounds, LagrangeBasisEvaluations, LookupSpec, OpeningProof, PolyComm, Radix2EvaluationDomain, srs_open, srs_verify,
 )

@@ -133,6 +133,11 @@ def lib() -> ctypes.CDLL:
     L.zk_poly_evaluate_chunks_dev.argtypes = [vp, i, ctypes.POINTER(DevPoly), sz, sz, sz, vp, sz, vp]
     L.zk_prover_ft_dev.argtypes = [vp, i, u, sz, ctypes.POINTER(LinTerm), sz, vp, sz, vp, vp, ctypes.POINTER(sz), vp]
     L.zk_perm_aggreg_dev.argtypes = [vp, i, u, sz, ctypes.POINTER(vp), ctypes.POINTER(vp), ctypes.c_uint64, vp, vp, vp, vp, vp, ctypes.POINTER(i)]
+    L.zk_lookup_joint_table_dev.argtypes = [vp, i, u, ctypes.POINTER(vp), sz, vp, vp, vp, vp, vp, vp]
+    L.zk_lookup_sorted_dev.argtypes = [vp, i, u, sz, ctypes.POINTER(vp), vp, u, ctypes.POINTER(LookupInfo), vp, ctypes.POINTER(vp),
+                                       ctypes.POINTER(ctypes.c_int64)]
+    L.zk_lookup_aggreg_dev.argtypes = [vp, i, u, sz, ctypes.POINTER(vp), vp, u, ctypes.POINTER(LookupInfo), ctypes.POINTER(vp), vp, vp, vp, vp,
+                                       ctypes.POINTER(i)]
     return L
 
 
@@ -168,6 +173,25 @@ class DevPoly(ctypes.Structure):
 class LinTerm(ctypes.Structure):
     """zk_lin_term (include/zkb200.h)"""
     _fields_ = [("d_evals", ctypes.c_void_p), ("len", ctypes.c_uint64), ("coeff", ctypes.c_uint64 * 4)]
+
+
+class LookupTerm(ctypes.Structure):
+    """zk_lookup_term (include/zkb200.h)"""
+    _fields_ = [("coeff", ctypes.c_uint64 * 4), ("column", ctypes.c_uint32), ("next", ctypes.c_uint32)]
+
+
+class LookupJoint(ctypes.Structure):
+    """zk_lookup_joint (include/zkb200.h)"""
+    _fields_ = [("table_id", ctypes.c_int32), ("table_id_column", ctypes.c_int32), ("n_entries", ctypes.c_uint32),
+                ("entry_terms", ctypes.c_uint32 * 4), ("first_term", ctypes.c_uint32)]
+
+
+class LookupInfo(ctypes.Structure):
+    """zk_lookup_info (include/zkb200.h); host.LookupSpec builds one"""
+    _fields_ = [("terms", ctypes.POINTER(LookupTerm)), ("n_terms", ctypes.c_size_t), ("lookups", ctypes.POINTER(LookupJoint)),
+                ("n_lookups", ctypes.c_size_t), ("pattern_first", ctypes.POINTER(ctypes.c_uint32)), ("pattern_count", ctypes.POINTER(ctypes.c_uint32)),
+                ("n_patterns", ctypes.c_size_t), ("row_pattern", ctypes.POINTER(ctypes.c_uint8)), ("max_per_row", ctypes.c_uint),
+                ("joint_combiner", ctypes.c_uint64 * 4), ("table_id_combiner", ctypes.c_uint64 * 4), ("dummy", ctypes.c_uint64 * 4)]
 
 
 class OpenPoly(ctypes.Structure):
@@ -479,6 +503,45 @@ class Context:
         ok = ctypes.c_int()
         check(lib().zk_perm_aggreg_dev(self._h, field, log_n, zk_rows, pw, ps, sigma_len, _ptr(b), _ptr(g), _ptr(sh), _ptr(rn),
                                        ctypes.c_void_p(d_z), ctypes.byref(ok)))
+        return bool(ok.value)
+
+    # ------------------------------------------------------------------ lookup argument (zk_lookup_*_dev)
+    def lookup_joint_table_dev(self, field: int, log_n: int, d_cols, joint_combiner, table_id_combiner, d_out8: int, d_table_ids8: int | None = None,
+                               d_runtime8: int | None = None, d_out1: int | None = None):
+        """zk_lookup_joint_table_dev: T8[i] = sum_c jc^c col_c[i] + tic tid8[i] over d8 from the resident columns d_cols (8 * 2^log_n
+        evaluations each; d_runtime8 is added to column 1), into d_out8 and, if given, its d1 values into d_out1.  Queued on the
+        context's stream."""
+        c = lambda a: np.ascontiguousarray(a, dtype=np.uint64).reshape(4)
+        jc, tic = c(joint_combiner), c(table_id_combiner)
+        cols = (ctypes.c_void_p * max(1, len(d_cols)))(*[int(p) for p in d_cols])
+        check(lib().zk_lookup_joint_table_dev(self._h, field, log_n, cols, len(d_cols), ctypes.c_void_p(d_table_ids8), ctypes.c_void_p(d_runtime8),
+                                              _ptr(jc), _ptr(tic), ctypes.c_void_p(d_out8), ctypes.c_void_p(d_out1)))
+
+    def lookup_sorted_dev(self, field: int, log_n: int, zk_rows: int, d_w, d_table: int, table_stride: int, info, rand, d_sorted) -> int:
+        """zk_lookup_sorted_dev (lookup::constraints::sorted + zk_patch): the max_per_row + 1 sorted columns (d1 evaluations) into
+        d_sorted from the 15 resident witness columns d_w and the joint table T1[i] = d_table[table_stride i].  info: a LookupInfo
+        structure (host.LookupSpec.info); rand: [(m + 1) * zk_rows, 4] Montgomery, column by column.  Returns -1, or the smallest row
+        whose lookup value is not in the table (ValueNotInTable; d_sorted is then untouched)."""
+        rn = np.ascontiguousarray(rand, dtype=np.uint64).reshape(-1)
+        pw = (ctypes.c_void_p * 15)(*[int(p) for p in d_w])
+        ps = (ctypes.c_void_p * max(1, len(d_sorted)))(*[int(p) for p in d_sorted])
+        row = ctypes.c_int64(-2)
+        check(lib().zk_lookup_sorted_dev(self._h, field, log_n, zk_rows, pw, ctypes.c_void_p(d_table), table_stride, ctypes.byref(info),
+                                         _ptr(rn) if rn.size else None, ps, ctypes.byref(row)))
+        return int(row.value)
+
+    def lookup_aggreg_dev(self, field: int, log_n: int, zk_rows: int, d_w, d_table: int, table_stride: int, info, d_sorted, beta, gamma, rand,
+                          d_aggreg: int) -> bool:
+        """zk_lookup_aggreg_dev (lookup::constraints::aggregation): the lookup aggregation polynomial's 2^log_n d1 evaluations into
+        d_aggreg; rand: [zk_rows, 4] Montgomery.  Returns whether agg[n - zk_rows - 1] == 1 (the reference's debug assertion)."""
+        c = lambda a: np.ascontiguousarray(a, dtype=np.uint64).reshape(4)
+        b, g = c(beta), c(gamma)
+        rn = np.ascontiguousarray(rand, dtype=np.uint64).reshape(-1)
+        pw = (ctypes.c_void_p * 15)(*[int(p) for p in d_w])
+        ps = (ctypes.c_void_p * max(1, len(d_sorted)))(*[int(p) for p in d_sorted])
+        ok = ctypes.c_int()
+        check(lib().zk_lookup_aggreg_dev(self._h, field, log_n, zk_rows, pw, ctypes.c_void_p(d_table), table_stride, ctypes.byref(info), ps,
+                                         _ptr(b), _ptr(g), _ptr(rn) if rn.size else None, ctypes.c_void_p(d_aggreg), ctypes.byref(ok)))
         return bool(ok.value)
 
     def points_fold_dev(self, curve: int, d_g: int, h: int, u_mont, d_out: int):

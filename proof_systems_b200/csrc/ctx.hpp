@@ -59,6 +59,8 @@ struct PinnedSlots {
     unsigned long long ft_len;  // zk_prover_ft_dev: ft's length and ft(zeta omega)
     fe ft_eval1;
     unsigned perm_final;        // zk_perm_aggreg_dev: z[n - zk_rows] == 1
+    unsigned lookup_sorted[2];  // zk_lookup_sorted_dev: the smallest row with a missing value (all ones: none), columns formed
+    unsigned lookup_final;      // zk_lookup_aggreg_dev: agg[n - zk_rows - 1] == 1
 };
 }  // namespace zkb
 
@@ -103,6 +105,8 @@ struct zk_ctx {
     zkb::DevScratch d_evals;             // zk_lagrange_evaluate_dev / zk_poly_evaluate_chunks_dev: descriptors | partial sums | results
     zkb::DevScratch d_ft;                // zk_prover_ft_dev: f over d1 | term descriptors | length counter
     zkb::DevScratch d_perm;              // zk_perm_aggreg_dev: den, then num / den over d1 | block products | final-value flag
+    zkb::DevScratch d_lookup;            // zk_lookup_sorted_dev / zk_lookup_aggreg_dev: lowered lookup info | random rows | the
+                                         // table's hash, counts and offsets, or the ratios and block products | flags
     uint64_t launches = 0;
     bool profile = false;                // per-stage device timing (zk_ctx_set_profile)
     std::atomic<bool> pinned{false};     // host-pointer calls stay on the primary lane (stream, profile, n_lanes; written under mu)

@@ -5,7 +5,8 @@
 //   r[j]   = num[j] / den[j], with 1 / 0 := 0 (ark_ff::batch_inversion skips zero entries and leaves them zero)
 //   z[0] = 1, z[j + 1] = z[j] r[j] for j < last           a multiplicative prefix scan over rows 0 .. last - 1:
 //                                                           k_perm_ratios (ratios, per-thread and per-block prefixes),
-//                                                           k_perm_block_scan (the block totals), k_perm_apply
+//                                                           k_block_product_scan (the block totals, prod_scan.cuh),
+//                                                           k_perm_apply
 //   z[last + 1] = rand0, z[last + 2] = rand1                the reference's two F::rand(rng) draws, in its order
 //   z[j + 1] = z[j] r[j] for j = last + 2 .. n - 2          zk_rows - 3 rows, one warp of k_perm_apply
 //   final value: z[last] == 1; z = interpolate(z) over d1   the library's inverse NTT, in place
@@ -16,6 +17,7 @@
 
 #include "../../include/zkb200.h"
 #include "ctx.hpp"
+#include "prod_scan.cuh"
 
 using namespace zkb;
 
@@ -40,30 +42,6 @@ struct PermAggArgs {
     fe beta, gamma;
     fe bshift[7];       // beta * shift_k
 };
-
-// exclusive prefix product of v over the block's threads (thread 0 gets one); *total: the product over all of them.  Every thread
-// of the block calls it.
-template <class FS> __device__ __forceinline__ fe block_exclusive_product(const fe& v, fe& total) {
-    __shared__ fe warp_tot[PA_THREADS / 32];
-    const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    fe incl = v;
-#pragma unroll
-    for (unsigned d = 1; d < 32; d <<= 1) {
-        const fe up = shfl_up_fe(incl, d);
-        if (lane >= d) incl = fe_mul<FS>(incl, up);
-    }
-    fe excl = shfl_up_fe(incl, 1);
-    if (lane == 0) excl = fe_one<FS>();
-    if (lane == 31) warp_tot[warp] = incl;
-    __syncthreads();
-    total = warp_tot[0];
-#pragma unroll
-    for (unsigned k = 1; k < PA_THREADS / 32; k++) {
-        if (k == warp) excl = fe_mul<FS>(excl, total);      // total is the product of the warps before this one here
-        total = fe_mul<FS>(total, warp_tot[k]);
-    }
-    return excl;
-}
 
 // rows [PA_ROWS t, PA_ROWS (t + 1)) of thread t: num and den, Montgomery's trick over the thread's nonzero den (one inversion),
 // r into a.r; the block's exclusive scan of the per-thread products below `last`; then z[j] = (product of r[i], i < j, within the
@@ -108,26 +86,11 @@ template <class FS> __global__ void __launch_bounds__(PA_THREADS) k_perm_ratios(
         }
     }
     fe block_total;
-    fe run = block_exclusive_product<FS>(tot, block_total);
+    fe run = block_exclusive_product<FS, PA_THREADS>(tot, block_total);
     if (threadIdx.x == 0) store_fe(a.block_tot + blockIdx.x, block_total);
     for (size_t j = j0; j < j1 && j <= a.last; j++) {
         store_fe(a.z + j, run);
         if (j < a.last) run = fe_mul<FS>(run, load_fe(a.r + j));
-    }
-}
-
-// one block: tot[b] <- product of tot[0 .. b - 1] (exclusive), each thread over a contiguous segment of the nb totals
-template <class FS> __global__ void __launch_bounds__(PA_THREADS) k_perm_block_scan(fe* tot, size_t nb) {
-    const size_t per = (nb + PA_THREADS - 1) / PA_THREADS;
-    const size_t b0 = threadIdx.x * per, b1 = b0 + per < nb ? b0 + per : nb;
-    fe p = fe_one<FS>();
-    for (size_t b = b0; b < b1; b++) p = fe_mul<FS>(p, load_fe(tot + b));
-    fe all;
-    fe run = block_exclusive_product<FS>(p, all);
-    for (size_t b = b0; b < b1; b++) {
-        const fe v = load_fe(tot + b);
-        store_fe(tot + b, run);
-        run = fe_mul<FS>(run, v);
     }
 }
 
@@ -212,7 +175,7 @@ static int perm_aggreg_impl(zk_ctx* ctx, unsigned log_n, size_t zk_rows, const v
     unsigned* d_flag = ctx->d_perm.at<unsigned>(o_flag);
     k_perm_ratios<FS><<<(unsigned)blocks, PA_THREADS, 0, st>>>(a);
     ZK_CUDA(cudaGetLastError());
-    k_perm_block_scan<FS><<<1, PA_THREADS, 0, st>>>(a.block_tot, blocks);
+    k_block_product_scan<FS, PA_THREADS><<<1, PA_THREADS, 0, st>>>(a.block_tot, blocks);
     ZK_CUDA(cudaGetLastError());
     k_perm_apply<FS><<<(unsigned)((last + PA_THREADS) / PA_THREADS + 1), PA_THREADS, 0, st>>>(d_z, a.block_tot, a.r, n, last, r0, r1, d_flag);
     ZK_CUDA(cudaGetLastError());

@@ -13,7 +13,7 @@ from dataclasses import dataclass
 
 import numpy as np
 
-from ._lib import BASE_FIELD, SCALAR_FIELD, Context, ZkError, _np_u64, _ptr, _u64p, check, lib
+from ._lib import BASE_FIELD, FP, FQ, SCALAR_FIELD, Context, ZkError, _np_u64, _ptr, _u64p, check, lib
 
 
 class BlindersDontMatch(ValueError):
@@ -411,6 +411,88 @@ class ExprProgram:
     def evaluations(self, ctx: Context, field: int, cols, out_len: int, out_domain_mult: int, d_out: int, accumulate: bool = False):
         """cols: [(device pointer, len, domain_mult)] in the order the program's cell() indices refer to"""
         ctx.expr_eval_dev(field, self.tokens, np.array(self.constants, dtype=np.uint64).reshape(-1, 4), cols, out_len, out_domain_mult, d_out, accumulate)
+
+
+_MONT_ONE = {FP: (0x34786d38fffffffd, 0x992c350be41914ad, 0xffffffffffffffff, 0x3fffffffffffffff),    # R mod p (host_field.hpp)
+             FQ: (0x5b2b3e9cfffffffd, 0x992c350be3420567, 0xffffffffffffffff, 0x3fffffffffffffff)}
+
+
+class LookupSpec:
+    """kimchi's LookupInfo lowered for zk_lookup_sorted_dev / zk_lookup_aggreg_dev: patterns of joint lookups (JointLookupSpec,
+    kimchi/src/circuits/lookup/lookups.rs:312-409) and, per call, each row's pattern (LookupInfo::by_row, :286-299).
+
+    A joint lookup is (table_id, entries): table_id an int (LookupTableID::Constant) or ("witness", column) (WitnessColumn, read at
+    the current row); entries up to 4 linear combinations (SingleLookup), each a list of terms (coeff, column, next_row) with coeff
+    Montgomery limbs [4] or None for one."""
+    XOR_TABLE_ID, RANGE_CHECK_TABLE_ID = 0, 1          # kimchi/src/circuits/lookup/tables/mod.rs:15-18
+    KIMCHI_PATTERNS = ("xor", "lookup", "range_check", "foreign_field_mul")
+
+    def __init__(self, field: int, max_per_row: int):
+        self.field, self.max_per_row = field, max_per_row
+        self.terms: list[tuple] = []
+        self.lookups: list[tuple] = []
+        self.patterns: list[tuple[int, int]] = []
+
+    @classmethod
+    def kimchi_lookups(cls, pattern: str) -> list:
+        """LookupPattern::lookups() (lookups.rs:448-528) of "xor", "lookup", "range_check" or "foreign_field_mul".  ForeignFieldMul
+        applies to its gate's row and the next one; that is the row mapping's business (by_row), not the pattern's."""
+        one = lambda col: [(None, col, False)]
+        if pattern == "xor":
+            return [(cls.XOR_TABLE_ID, [one(3 + i), one(7 + i), one(11 + i)]) for i in range(4)]
+        if pattern == "lookup":
+            return [(("witness", 0), [one(2 * i + 1), one(2 * i + 2)]) for i in range(3)]
+        if pattern == "range_check":
+            return [(cls.RANGE_CHECK_TABLE_ID, [one(c)]) for c in range(3, 7)]
+        if pattern == "foreign_field_mul":
+            return [(cls.RANGE_CHECK_TABLE_ID, [one(c)]) for c in range(7, 11)]
+        raise ValueError(f"unknown lookup pattern {pattern!r}")
+
+    def add_pattern(self, lookups) -> int:
+        """Appends a pattern (a list of joint lookups); returns its index p — rows using it carry p + 1 in row_pattern"""
+        first = len(self.lookups)
+        for table_id, entries in lookups:
+            first_term = len(self.terms)
+            counts = []
+            for entry in entries:
+                for coeff, col, nxt in entry:
+                    self.terms.append((_MONT_ONE[self.field] if coeff is None else tuple(int(x) for x in np.asarray(coeff, dtype=np.uint64).reshape(4)),
+                                       int(col), int(bool(nxt))))
+                counts.append(len(entry))
+            tid, tcol = (0, int(table_id[1])) if isinstance(table_id, tuple) else (int(table_id), -1)
+            self.lookups.append((tid, tcol, counts, first_term))
+        self.patterns.append((first, len(lookups)))
+        return len(self.patterns) - 1
+
+    def add_kimchi_pattern(self, pattern: str) -> int:
+        return self.add_pattern(self.kimchi_lookups(pattern))
+
+    def info(self, row_pattern, joint_combiner, table_id_combiner, dummy) -> "LookupInfo":
+        """The zk_lookup_info of these patterns for rows row_pattern (uint8 [lookup_rows]: 0 none, p + 1 pattern p); scalars Montgomery"""
+        from ._lib import LookupInfo, LookupJoint, LookupTerm
+        terms = (LookupTerm * max(1, len(self.terms)))()
+        for k, (c, col, nxt) in enumerate(self.terms):
+            terms[k].coeff[:] = list(c)
+            terms[k].column, terms[k].next = col, nxt
+        joints = (LookupJoint * max(1, len(self.lookups)))()
+        for k, (tid, tcol, counts, first_term) in enumerate(self.lookups):
+            joints[k].table_id, joints[k].table_id_column, joints[k].first_term = tid, tcol, first_term
+            joints[k].n_entries = len(counts)                    # more than 4: the library refuses the call
+            for e, cnt in enumerate(counts[:4]):
+                joints[k].entry_terms[e] = cnt
+        first = (ctypes.c_uint32 * max(1, len(self.patterns)))(*[p[0] for p in self.patterns])
+        count = (ctypes.c_uint32 * max(1, len(self.patterns)))(*[p[1] for p in self.patterns])
+        rows = np.ascontiguousarray(row_pattern, dtype=np.uint8)
+        s = LookupInfo()
+        s.terms, s.n_terms = ctypes.cast(terms, ctypes.POINTER(LookupTerm)), len(self.terms)
+        s.lookups, s.n_lookups = ctypes.cast(joints, ctypes.POINTER(LookupJoint)), len(self.lookups)
+        s.pattern_first, s.pattern_count, s.n_patterns = ctypes.cast(first, ctypes.POINTER(ctypes.c_uint32)), ctypes.cast(count, ctypes.POINTER(ctypes.c_uint32)), len(self.patterns)
+        s.row_pattern = rows.ctypes.data_as(ctypes.POINTER(ctypes.c_uint8))
+        s.max_per_row = self.max_per_row
+        for name, v in (("joint_combiner", joint_combiner), ("table_id_combiner", table_id_combiner), ("dummy", dummy)):
+            getattr(s, name)[:] = [int(x) for x in np.asarray(v, dtype=np.uint64).reshape(4)]
+        s._keep = (terms, joints, first, count, rows)          # the arrays the structure points into
+        return s
 
 
 class LagrangeBasisEvaluations:
