@@ -58,10 +58,15 @@ struct PinnedSlots {
     unsigned remainder;         // zk_poly_divide_by_vanishing_dev: nonzero remainder flag
     unsigned long long ft_len;  // zk_prover_ft_dev: ft's length and ft(zeta omega)
     fe ft_eval1;
-    unsigned perm_final;        // zk_perm_aggreg_dev: z[n - zk_rows] == 1
+    unsigned agg_final;         // zk_perm_aggreg_dev / zk_lookup_aggreg_dev: z[n - zk_rows] == 1 / agg[n - zk_rows - 1] == 1
     unsigned lookup_sorted[2];  // zk_lookup_sorted_dev: the smallest row with a missing value (all ones: none), columns formed
-    unsigned lookup_final;      // zk_lookup_aggreg_dev: agg[n - zk_rows - 1] == 1
 };
+
+// [p, p + bytes) and [q, q + qbytes) share a byte
+inline bool overlaps(const void* p, size_t bytes, const void* q, size_t qbytes) {
+    const uintptr_t a = (uintptr_t)p, b = (uintptr_t)q;
+    return a < b + qbytes && b < a + bytes;
+}
 }  // namespace zkb
 
 struct zk_ctx {

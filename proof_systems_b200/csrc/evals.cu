@@ -72,7 +72,7 @@ template <class FS> __global__ void __launch_bounds__(EV_THREADS) k_sum_partials
 
 // ------------------------------------------------------------------------------------------------ basis, n <= max_poly_size
 struct LagBasisArgs {
-    const fe* ulo;      // w^-i = ulo[i & 1023] * mid[(i >> 10) & 1023] * hi2[i >> 20]  (inverse transform's unscaled tables)
+    const fe* ulo;      // w^-i from the inverse transform's unscaled tables (domain_point, ntt.cuh)
     const fe* mid;
     const fe* hi2;
     fe* out;
@@ -83,9 +83,7 @@ struct LagBasisArgs {
 };
 
 template <class FS> __device__ __forceinline__ fe lag_denominator(const LagBasisArgs& a, size_t i) {
-    fe w = load_fe_nc(a.ulo + (i & 1023));
-    if ((i >> 10) & 1023) w = fe_mul<FS>(w, load_fe_nc(a.mid + ((i >> 10) & 1023)));
-    if (i >> 20) w = fe_mul<FS>(w, load_fe_nc(a.hi2 + (i >> 20)));
+    const fe w = domain_point<FS>(a.ulo, a.mid, a.hi2, i);
     return fe_sub<FS>(fe_mul<FS>(a.x, w), fe_one<FS>());       // x w^-i - 1 = w^-i (x - w^i)
 }
 

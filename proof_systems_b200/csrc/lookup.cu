@@ -10,28 +10,23 @@
 //   k_lookup_count    one thread per (row, lookup slot): the joint value f, probed in the hash; count[first] += 1 (aggregated
 //                     over the warp's lanes that hit the same row), a miss takes atomicMin(bad_row, i); padded slots are counted
 //   k_lookup_pad      count[first(dummy)] += padding; whether the columns can be formed
-//   k_lookup_offsets_block, _top, _apply   offsets = exclusive sum of c_r = 1 + count[r] (three launches)
+//   k_lookup_offsets_block, k_scan_block_totals (scan.cuh), k_lookup_offsets_apply   offsets = exclusive sum of c_r = 1 + count[r]
 //   k_lookup_place    one thread per output element: its position in the pre-snake sequence, a binary search of the offsets for
 //                     the table row, T1[r] (or the caller's random value in the zk rows); nothing when a value was missing
-// Aggregation (lookup/constraints.rs:233-338), the shape of perm.cu: 16 rows per thread, den over the m + 1 sorted columns inverted
-// with Montgomery's trick (a zero den stays zero), f and t recomputed from the witness and the table, then a multiplicative
-// prefix scan in three launches (prod_scan.cuh).  No kernel waits on another CTA.  Field arithmetic is exact, so every association
-// order gives the reference's bits.
+// Aggregation (lookup/constraints.rs:233-338), aggreg.cuh with end = L + 1 and last = L (LookupRows): den over the m + 1 sorted
+// columns, f and t recomputed from the witness and the table, ratio one at position L; the tail copies the zk_rows random rows.
 #include <cstring>
 #include <mutex>
 #include <vector>
 
 #include "../../include/zkb200.h"
-#include "ctx.hpp"
-#include "prod_scan.cuh"
+#include "aggreg.cuh"
 
 using namespace zkb;
 
 namespace zkb {
 
 constexpr unsigned LK_THREADS = 128;                        // every kernel below: 4 warps
-constexpr unsigned LK_ROWS = 16;                            // aggregation rows per thread (one inversion each)
-constexpr unsigned LK_BLOCK_ROWS = LK_THREADS * LK_ROWS;
 constexpr unsigned LK_SCAN_ITEMS = 16;                      // table rows per thread of the offset scan
 constexpr unsigned LK_SCAN_BLOCK = LK_THREADS * LK_SCAN_ITEMS;
 constexpr unsigned LK_MAX_COLS = 16;                        // joint table columns
@@ -183,28 +178,6 @@ __global__ void k_lookup_pad(const uint32_t* slots, unsigned log_h, const fe* T,
     flags[F_OK] = flags[F_BAD_ROW] == LK_EMPTY && formed ? 1u : 0u;
 }
 
-// exclusive prefix sum of v over the block's threads; *total: the sum over all of them
-__device__ __forceinline__ uint32_t block_exclusive_sum(uint32_t v, uint32_t& total) {
-    __shared__ uint32_t warp_tot[LK_THREADS / 32];
-    const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint32_t incl = v;
-#pragma unroll
-    for (unsigned d = 1; d < 32; d <<= 1) {
-        const uint32_t up = __shfl_up_sync(0xffffffffu, incl, d);
-        if (lane >= d) incl += up;
-    }
-    if (lane == 31) warp_tot[warp] = incl;
-    __syncthreads();
-    uint32_t before = 0;
-    total = 0;
-#pragma unroll
-    for (unsigned k = 0; k < LK_THREADS / 32; k++) {
-        if (k < warp) before += warp_tot[k];
-        total += warp_tot[k];
-    }
-    return before + incl - v;
-}
-
 // off[r] = sum of c_q = 1 + count[q] over the block's q < r; btot[b] = the block's sum.  (m + 1) L < 2^32 bounds every sum.
 __global__ void __launch_bounds__(LK_THREADS) k_lookup_offsets_block(const uint32_t* __restrict__ count, uint32_t* off, uint32_t* btot, size_t L) {
     const size_t r0 = ((size_t)blockIdx.x * LK_THREADS + threadIdx.x) * LK_SCAN_ITEMS;
@@ -212,26 +185,11 @@ __global__ void __launch_bounds__(LK_THREADS) k_lookup_offsets_block(const uint3
     uint32_t sum = 0;
     for (size_t r = r0; r < r1; r++) sum += 1 + count[r];
     uint32_t total;
-    uint32_t run = block_exclusive_sum(sum, total);
+    uint32_t run = block_exclusive_scan<AddU32, LK_THREADS>(sum, total);
     if (threadIdx.x == 0) btot[blockIdx.x] = total;
     for (size_t r = r0; r < r1; r++) {
         off[r] = run;
         run += 1 + count[r];
-    }
-}
-
-// one block: btot[b] <- sum of btot[0 .. b - 1]
-__global__ void __launch_bounds__(LK_THREADS) k_lookup_offsets_top(uint32_t* btot, size_t nb) {
-    const size_t per = (nb + LK_THREADS - 1) / LK_THREADS;
-    const size_t b0 = threadIdx.x * per, b1 = b0 + per < nb ? b0 + per : nb;
-    uint32_t sum = 0;
-    for (size_t b = b0; b < b1; b++) sum += btot[b];
-    uint32_t total;
-    uint32_t run = block_exclusive_sum(sum, total);
-    for (size_t b = b0; b < b1; b++) {
-        const uint32_t v = btot[b];
-        btot[b] = run;
-        run += v;
     }
 }
 
@@ -275,94 +233,47 @@ __global__ void __launch_bounds__(LK_THREADS) k_lookup_place(const __grid_consta
 }
 
 // ------------------------------------------------------------------------------------------------------------ aggregation
-struct AggArgs {
+template <class FS> struct LookupRows {
     LookupSpec s;
     const fe* T;
     const fe* sorted[LK_MAX_M + 1];
-    fe* agg;             // the caller's buffer: num * (product of the thread's earlier nonzero den), then the block-local prefixes
-    fe* r;               // scratch, L + 1: den, then num / den
-    fe* block_tot;
     size_t stride, L;
     fe beta, gamma, gb1; // gb1 = gamma (1 + beta)
     fe pad_pow[LK_MAX_M + 1];   // (1 + beta)^m (gamma + dummy)^k
+
+    struct Cursor {};
+    __device__ Cursor start(size_t) const { return {}; }
+    // positions 0 .. L; position L: ratio one, it only receives agg[L]
+    __device__ void row(Cursor&, size_t j, fe& num, fe& den) const {
+        num = den = fe_one<FS>();
+        if (j == L) return;
+#pragma unroll 1
+        for (unsigned k = 0; k <= s.m; k++) {
+            const fe sa = load_fe_nc(sorted[k] + j + (k & 1)), sb = load_fe_nc(sorted[k] + j + 1 - (k & 1));
+            den = fe_mul<FS>(den, fe_add<FS>(fe_add<FS>(gb1, sa), fe_mul<FS>(beta, sb)));
+        }
+        const unsigned p = s.row_pattern[j];
+        const DevPattern pat = p ? s.patterns[p - 1] : DevPattern{0, 0};
+        num = pad_pow[s.m - pat.count];
+#pragma unroll 1
+        for (unsigned q = 0; q < pat.count; q++)
+            num = fe_mul<FS>(num, fe_add<FS>(gamma, joint_value<FS>(s, s.joints[pat.first + q], j)));
+        const fe t0 = load_fe_nc(T + stride * j), t1 = load_fe_nc(T + stride * (j + 1));
+        num = fe_mul<FS>(num, fe_add<FS>(fe_add<FS>(gb1, t0), fe_mul<FS>(beta, t1)));
+    }
 };
 
-// rows [LK_ROWS t, LK_ROWS (t + 1)) of thread t over positions 0 .. L (position L: ratio one, it only receives agg[L])
-template <class FS> __global__ void __launch_bounds__(LK_THREADS) k_lookup_ratios(const __grid_constant__ AggArgs a) {
-    const size_t j0 = ((size_t)blockIdx.x * LK_THREADS + threadIdx.x) * LK_ROWS;
-    const size_t j1 = j0 + LK_ROWS < a.L + 1 ? j0 + LK_ROWS : a.L + 1;
-    fe tot = fe_one<FS>();
-    if (j0 < j1) {
-        fe acc = fe_one<FS>();
-        for (size_t j = j0; j < j1; j++) {
-            fe num = fe_one<FS>(), den = fe_one<FS>();
-            if (j < a.L) {
-#pragma unroll 1
-                for (unsigned k = 0; k <= a.s.m; k++) {
-                    const fe sa = load_fe_nc(a.sorted[k] + j + (k & 1)), sb = load_fe_nc(a.sorted[k] + j + 1 - (k & 1));
-                    den = fe_mul<FS>(den, fe_add<FS>(fe_add<FS>(a.gb1, sa), fe_mul<FS>(a.beta, sb)));
-                }
-                const unsigned p = a.s.row_pattern[j];
-                const DevPattern pat = p ? a.s.patterns[p - 1] : DevPattern{0, 0};
-                num = a.pad_pow[a.s.m - pat.count];
-#pragma unroll 1
-                for (unsigned q = 0; q < pat.count; q++)
-                    num = fe_mul<FS>(num, fe_add<FS>(a.gamma, joint_value<FS>(a.s, a.s.joints[pat.first + q], j)));
-                const fe t0 = load_fe_nc(a.T + a.stride * j), t1 = load_fe_nc(a.T + a.stride * (j + 1));
-                num = fe_mul<FS>(num, fe_add<FS>(fe_add<FS>(a.gb1, t0), fe_mul<FS>(a.beta, t1)));
-            }
-            store_fe(a.agg + j, fe_mul<FS>(num, acc));
-            store_fe(a.r + j, den);
-            if (!fe_is_zero(den)) acc = fe_mul<FS>(acc, den);
-        }
-        fe inv = fe_inv<FS>(acc);
-        for (size_t j = j1; j-- > j0;) {
-            const fe den = load_fe(a.r + j);
-            fe r = fe_zero();
-            if (!fe_is_zero(den)) {
-                r = fe_mul<FS>(inv, load_fe(a.agg + j));
-                inv = fe_mul<FS>(inv, den);
-            }
-            store_fe(a.r + j, r);
-            if (j < a.L) tot = fe_mul<FS>(tot, r);
-        }
-    }
-    fe block_total;
-    fe run = block_exclusive_product<FS, LK_THREADS>(tot, block_total);
-    if (threadIdx.x == 0) store_fe(a.block_tot + blockIdx.x, block_total);
-    for (size_t j = j0; j < j1; j++) {
-        store_fe(a.agg + j, run);
-        if (j < a.L) run = fe_mul<FS>(run, load_fe(a.r + j));
-    }
-}
-
-// blocks 0 .. gridDim.x - 2: agg[j] *= tot[j / LK_BLOCK_ROWS] for j <= L, and the flag agg[L] == 1; the last block's first warp:
 // agg[L + 1 + q] = rand[q], q < zk_rows
-template <class FS> __global__ void __launch_bounds__(LK_THREADS) k_lookup_agg_apply(fe* agg, const fe* __restrict__ tot, const fe* __restrict__ rand,
-                                                                                    size_t L, size_t zk_rows, unsigned* final_is_one) {
-    if (blockIdx.x + 1 < gridDim.x) {
-        const size_t j = (size_t)blockIdx.x * LK_THREADS + threadIdx.x;
-        if (j > L) return;
-        fe v = load_fe(agg + j);
-        const size_t b = j / LK_BLOCK_ROWS;
-        if (b) {
-            v = fe_mul<FS>(v, load_fe_nc(tot + b));
-            store_fe(agg + j, v);
-        }
-        if (j == L) *final_is_one = fe_eq(v, fe_one<FS>()) ? 1u : 0u;
-        return;
+struct LookupTail {
+    const fe* rand;
+    size_t zk_rows;
+
+    __device__ void operator()(fe* agg, size_t L, unsigned lane) const {
+        for (size_t q = lane; q < zk_rows; q += 32) store_fe(agg + L + 1 + q, load_fe_nc(rand + q));
     }
-    if (threadIdx.x >= 32) return;
-    for (size_t q = threadIdx.x; q < zk_rows; q += 32) store_fe(agg + L + 1 + q, load_fe_nc(rand + q));
-}
+};
 
 // ------------------------------------------------------------------------------------------------------------ host side
-// [p, p + bytes) and [q, q + qbytes) share a byte
-static bool overlaps(const void* p, size_t bytes, const void* q, size_t qbytes) {
-    const uintptr_t a = (uintptr_t)p, b = (uintptr_t)q;
-    return a < b + qbytes && b < a + bytes;
-}
-
 // zk_lookup_info checked against a table of L lookup rows
 static int check_info(const char* what, int field_id, size_t L, const zk_lookup_info* info) {
     if (!info->row_pattern || (info->n_terms && !info->terms) || (info->n_lookups && !info->lookups) ||
@@ -555,7 +466,7 @@ static int sorted_impl(zk_ctx* ctx, unsigned log_n, size_t zk_rows, const void* 
     ZK_CUDA(cudaGetLastError());
     k_lookup_offsets_block<<<(unsigned)nb, LK_THREADS, 0, st>>>(count, off, btot, L);
     ZK_CUDA(cudaGetLastError());
-    k_lookup_offsets_top<<<1, LK_THREADS, 0, st>>>(btot, nb);
+    k_scan_block_totals<AddU32, LK_THREADS><<<1, LK_THREADS, 0, st>>>(btot, nb);
     ZK_CUDA(cudaGetLastError());
     k_lookup_offsets_apply<<<(unsigned)blocks_for(L, LK_THREADS), LK_THREADS, 0, st>>>(off, btot, L);
     ZK_CUDA(cudaGetLastError());
@@ -588,9 +499,9 @@ static int aggreg_impl(zk_ctx* ctx, unsigned log_n, size_t zk_rows, const void* 
     using FS = typename T::Dev; using HP = typename T::Host;
     const size_t n = (size_t)1 << log_n, L = n - zk_rows - 1;
     const unsigned m = info->max_per_row;
-    AggArgs a{};
+    LookupRows<FS> a{};
     for (unsigned k = 0; k <= m; k++) a.sorted[k] = (const fe*)d_sorted[k];
-    a.T = T1; a.agg = d_agg; a.stride = stride; a.L = L;
+    a.T = T1; a.stride = stride; a.L = L;
     hfe hb, hg, hd;
     memcpy(hb.l, beta, 32);
     memcpy(hg.l, gamma, 32);
@@ -612,29 +523,21 @@ static int aggreg_impl(zk_ctx* ctx, unsigned log_n, size_t zk_rows, const void* 
     PinnedSlots* pin = ctx_pinned(ctx);
     if (!pin) return ZK_ERR_CUDA;
     // context scratch: lowered info | random rows | ratios over positions 0 .. L | block products | final-value flag
-    const size_t blocks = blocks_for(L + 1, LK_BLOCK_ROWS);
     Layout lay;
     StagedInfo si;
     lower_info<T>(info, L, rand, zk_rows, lay, si);
-    const size_t o_r = lay.add((L + 1) * sizeof(fe)), o_tot = lay.add(blocks * sizeof(fe)), o_flag = lay.add(sizeof(unsigned));
+    const size_t o_r = lay.add((L + 1) * sizeof(fe)), o_tot = lay.add(agg_blocks(L + 1) * sizeof(fe)), o_flag = lay.add(sizeof(unsigned));
     int rc = ctx->d_lookup.ensure(lay.total);
     if (rc) return rc;
     rc = upload_info(ctx, st, si, info, d_w, a.s);
     if (rc) return rc;
-    a.r = ctx->d_lookup.at<fe>(o_r);
-    a.block_tot = ctx->d_lookup.at<fe>(o_tot);
     unsigned* d_flag = ctx->d_lookup.at<unsigned>(o_flag);
-    k_lookup_ratios<FS><<<(unsigned)blocks, LK_THREADS, 0, st>>>(a);
-    ZK_CUDA(cudaGetLastError());
-    k_block_product_scan<FS, LK_THREADS><<<1, LK_THREADS, 0, st>>>(a.block_tot, blocks);
-    ZK_CUDA(cudaGetLastError());
-    k_lookup_agg_apply<FS><<<(unsigned)((L + LK_THREADS) / LK_THREADS + 1), LK_THREADS, 0, st>>>(d_agg, a.block_tot, ctx->d_lookup.at<fe>(si.o_extra), L,
-                                                                                              zk_rows, d_flag);
-    ZK_CUDA(cudaGetLastError());
-    ctx->launches += 3;
-    ZK_CUDA(cudaMemcpyAsync(&pin->lookup_final, d_flag, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    const LookupTail tail{ctx->d_lookup.at<fe>(si.o_extra), zk_rows};
+    rc = agg_launch<FS>(ctx, a, tail, d_agg, ctx->d_lookup.at<fe>(o_r), ctx->d_lookup.at<fe>(o_tot), L + 1, L, d_flag);
+    if (rc) return rc;
+    ZK_CUDA(cudaMemcpyAsync(&pin->agg_final, d_flag, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
     ZK_CUDA(cudaStreamSynchronize(st));
-    *final_is_one = pin->lookup_final ? 1 : 0;
+    *final_is_one = pin->agg_final ? 1 : 0;
     return ZK_OK;
 }
 

@@ -200,10 +200,7 @@ template <class F> __global__ void __launch_bounds__(128, 6) k_ntt_pass(NttPassP
                 v = fe_mul<F>(v, tw[u]);
             } else if (p.lo) {
                 const unsigned e = (unsigned)tw_col * k;                  // < 2^30
-                fe t = load_fe_nc(p.lo + (e & 1023));
-                if ((e >> 10) & 1023) t = fe_mul<F>(t, load_fe_nc(p.mid + ((e >> 10) & 1023)));
-                if (e >> 20) t = fe_mul<F>(t, load_fe_nc(p.hi2 + (e >> 20)));
-                v = fe_mul<F>(v, t);
+                v = fe_mul<F>(v, domain_point<F>(p.lo, p.mid, p.hi2, e));
             }
             if (p.scale) v = fe_mul<F>(v, load_fe_nc(p.scale));
             store_fe(out + k * p.out_rs, v);

@@ -38,6 +38,16 @@ struct NttTables {
     DevScratch full;     // [n]    w_n^(+-(col * k)) (inverse: times n^-1) at index col * n1 + k: contiguous per tile of pass 1; empty outside 2^10 < n <= 2^20
 };
 
+// w^e = lo[e & 1023] * mid[(e >> 10) & 1023] * hi2[e >> 20] from a transform's three 1024-entry tables (lo, or ulo for the
+// unscaled powers), e < 2^30.  I: the index type of the caller's arithmetic.  e is taken by reference: taken by value, nvcc
+// (12.9) tests the table indices in another form and the callers' SASS changes.
+template <class F, class I> __device__ __forceinline__ fe domain_point(const fe* lo, const fe* mid, const fe* hi2, const I& e) {
+    fe x = load_fe_nc(lo + (e & 1023));
+    if ((e >> 10) & 1023) x = fe_mul<F>(x, load_fe_nc(mid + ((e >> 10) & 1023)));
+    if (e >> 20) x = fe_mul<F>(x, load_fe_nc(hi2 + (e >> 20)));
+    return x;
+}
+
 // One pass = independent S-point transforms of columns ("tiles").  Tile tau = (t_hi << split_log) | t_lo of polynomial b reads
 //     in[b * in_bs + t_hi * in_hi + t_lo * in_lo + r * in_rs],  r < S        (zero where the position is >= in_len)
 // and writes X[k] (natural order) times the pass twiddle to out[b * out_bs + t_hi * out_hi + t_lo * out_lo + k * out_rs].
@@ -47,7 +57,7 @@ struct NttPassParams {
     const fe* small;       // [512] w_1024^(+-i)
     const fe* tw_full;     // pass twiddle: n-entry table, entry (tau << log_s) + k, or
     const fe* lo;          //               three 1024-entry tables, exponent e = (tw_by_lo ? t_lo : tau) * k,
-    const fe* mid;         //               w^e = lo[e & 1023] * mid[(e >> 10) & 1023] * hi2[e >> 20]; all null: no twiddle
+    const fe* mid;         //               w^e = domain_point(lo, mid, hi2, e); all null: no twiddle
     const fe* hi2;
     const fe* scale;       // optional factor applied at the store (device pointer, e.g. n^-1), or null
     unsigned log_s;        // sub-transform size S = 2^log_s

@@ -2,136 +2,73 @@
 // the device, from the resident witness and permutation_coefficients8, so z never has to be built on the host and uploaded.
 // With n = |d1|, last = n - zk_rows and sid[j] = omega^j:
 //   num[j] = prod_{k<7} (w_k[j] + beta shift_k omega^j + gamma)      den[j] = prod_{k<7} (w_k[j] + beta sigma_k[s j] + gamma)
-//   r[j]   = num[j] / den[j], with 1 / 0 := 0 (ark_ff::batch_inversion skips zero entries and leaves them zero)
-//   z[0] = 1, z[j + 1] = z[j] r[j] for j < last           a multiplicative prefix scan over rows 0 .. last - 1:
-//                                                           k_perm_ratios (ratios, per-thread and per-block prefixes),
-//                                                           k_block_product_scan (the block totals, prod_scan.cuh),
-//                                                           k_perm_apply
+//   r[j]   = num[j] / den[j] for j < n, z[0] = 1, z[j + 1] = z[j] r[j] for j < last, the flag z[last] == 1:
+//                                                           aggreg.cuh with end = n (PermRows)
 //   z[last + 1] = rand0, z[last + 2] = rand1                the reference's two F::rand(rng) draws, in its order
-//   z[j + 1] = z[j] r[j] for j = last + 2 .. n - 2          zk_rows - 3 rows, one warp of k_perm_apply
-//   final value: z[last] == 1; z = interpolate(z) over d1   the library's inverse NTT, in place
-// No kernel waits on another CTA: the scan's three levels are three launches.  Field arithmetic is exact, so this association
-// order gives the reference's bits.
+//   z[j + 1] = z[j] r[j] for j = last + 2 .. n - 2          zk_rows - 3 rows, a warp scan (PermTail)
+//   z = interpolate(z) over d1                              the library's inverse NTT, in place
 #include <cstring>
 #include <mutex>
 
 #include "../../include/zkb200.h"
-#include "ctx.hpp"
-#include "prod_scan.cuh"
+#include "aggreg.cuh"
 
 using namespace zkb;
 
 namespace zkb {
 
-constexpr unsigned PA_THREADS = 128;                       // every kernel below: 4 warps
-constexpr unsigned PA_ROWS = 16;                           // consecutive rows per thread of k_perm_ratios (one inversion each)
-constexpr unsigned PA_BLOCK_ROWS = PA_THREADS * PA_ROWS;   // rows per block, one block total each
-
-struct PermAggArgs {
+template <class FS> struct PermRows {
     const fe* w[7];     // witness columns over d1
     const fe* sigma[7]; // permutation_coefficients8 (or any s n evaluations), read at s j
-    const fe* ulo;      // omega^j from the forward transform's tables (ntt.cuh): ulo[j & 1023] * mid[(j >> 10) & 1023] * hi2[j >> 20]
+    const fe* ulo;      // omega^j from the forward transform's tables (domain_point, ntt.cuh)
     const fe* mid;
     const fe* hi2;
-    fe* z;              // the caller's buffer: num * (product of the thread's earlier nonzero den), then the block-local prefixes
-    fe* r;              // scratch, n: den, then r = num / den for every row (the tail reads its rows from here)
-    fe* block_tot;      // scratch: each block's product of r over its rows below `last`
-    size_t n;
-    size_t last;        // n - zk_rows
     size_t sigma_stride;
     fe beta, gamma;
     fe bshift[7];       // beta * shift_k
+
+    struct Cursor { fe x, omega; };     // x = omega^j
+    __device__ Cursor start(size_t j0) const { return {domain_point<FS>(ulo, mid, hi2, j0), load_fe_nc(ulo + 1)}; }
+    __device__ void row(Cursor& c, size_t j, fe& num, fe& den) const {
+        fe wg = fe_add<FS>(load_fe_nc(w[0] + j), gamma);
+        num = fe_add<FS>(wg, fe_mul<FS>(c.x, bshift[0]));
+        den = fe_add<FS>(wg, fe_mul<FS>(beta, load_fe_nc(sigma[0] + sigma_stride * j)));
+#pragma unroll 1
+        for (unsigned k = 1; k < 7; k++) {
+            wg = fe_add<FS>(load_fe_nc(w[k] + j), gamma);
+            num = fe_mul<FS>(num, fe_add<FS>(wg, fe_mul<FS>(c.x, bshift[k])));
+            den = fe_mul<FS>(den, fe_add<FS>(wg, fe_mul<FS>(beta, load_fe_nc(sigma[k] + sigma_stride * j))));
+        }
+        c.x = fe_mul<FS>(c.x, c.omega);
+    }
 };
 
-// rows [PA_ROWS t, PA_ROWS (t + 1)) of thread t: num and den, Montgomery's trick over the thread's nonzero den (one inversion),
-// r into a.r; the block's exclusive scan of the per-thread products below `last`; then z[j] = (product of r[i], i < j, within the
-// block) for j <= last.  Block totals go to a.block_tot.
-template <class FS> __global__ void __launch_bounds__(PA_THREADS) k_perm_ratios(const __grid_constant__ PermAggArgs a) {
-    const size_t j0 = ((size_t)blockIdx.x * PA_THREADS + threadIdx.x) * PA_ROWS;
-    const size_t j1 = j0 + PA_ROWS < a.n ? j0 + PA_ROWS : a.n;
-    fe tot = fe_one<FS>();
-    if (j0 < a.n) {
-        // forward: z[j] = num[j] * (product of the nonzero den[i], j0 <= i < j), r[j] = den[j]
-        fe x = load_fe_nc(a.ulo + (j0 & 1023));
-        if ((j0 >> 10) & 1023) x = fe_mul<FS>(x, load_fe_nc(a.mid + ((j0 >> 10) & 1023)));
-        if (j0 >> 20) x = fe_mul<FS>(x, load_fe_nc(a.hi2 + (j0 >> 20)));
-        const fe omega = load_fe_nc(a.ulo + 1);
-        fe acc = fe_one<FS>();
-        for (size_t j = j0; j < j1; j++) {
-            fe wg = fe_add<FS>(load_fe_nc(a.w[0] + j), a.gamma);
-            fe num = fe_add<FS>(wg, fe_mul<FS>(x, a.bshift[0]));
-            fe den = fe_add<FS>(wg, fe_mul<FS>(a.beta, load_fe_nc(a.sigma[0] + a.sigma_stride * j)));
-#pragma unroll 1
-            for (unsigned k = 1; k < 7; k++) {
-                wg = fe_add<FS>(load_fe_nc(a.w[k] + j), a.gamma);
-                num = fe_mul<FS>(num, fe_add<FS>(wg, fe_mul<FS>(x, a.bshift[k])));
-                den = fe_mul<FS>(den, fe_add<FS>(wg, fe_mul<FS>(a.beta, load_fe_nc(a.sigma[k] + a.sigma_stride * j))));
-            }
-            store_fe(a.z + j, fe_mul<FS>(num, acc));
-            store_fe(a.r + j, den);
-            if (!fe_is_zero(den)) acc = fe_mul<FS>(acc, den);
-            x = fe_mul<FS>(x, omega);
-        }
-        // backward: inv = 1 / (product of the nonzero den[i], j0 <= i <= j), so r[j] = inv * z[j]; a zero den gives r[j] = 0
-        fe inv = fe_inv<FS>(acc);
-        for (size_t j = j1; j-- > j0;) {
-            const fe den = load_fe(a.r + j);
-            fe r = fe_zero();
-            if (!fe_is_zero(den)) {
-                r = fe_mul<FS>(inv, load_fe(a.z + j));
-                inv = fe_mul<FS>(inv, den);
-            }
-            store_fe(a.r + j, r);
-            if (j < a.last) tot = fe_mul<FS>(tot, r);
-        }
-    }
-    fe block_total;
-    fe run = block_exclusive_product<FS, PA_THREADS>(tot, block_total);
-    if (threadIdx.x == 0) store_fe(a.block_tot + blockIdx.x, block_total);
-    for (size_t j = j0; j < j1 && j <= a.last; j++) {
-        store_fe(a.z + j, run);
-        if (j < a.last) run = fe_mul<FS>(run, load_fe(a.r + j));
-    }
-}
+// z[last + 1] = rand0, z[last + 2] = rand1, then z[j + 1] = z[j] r[j] for j = last + 2 .. n - 2 as a warp scan, 32 rows per step
+template <class FS> struct PermTail {
+    const fe* r;
+    size_t n;
+    fe rand0, rand1;
 
-// blocks 0 .. gridDim.x - 2: z[j] *= tot[j / PA_BLOCK_ROWS] for j <= last, and the final-value flag z[last] == 1;
-// the last block's first warp: z[last + 1] = rand0, z[last + 2] = rand1, then z[j + 1] = z[j] r[j] for j = last + 2 .. n - 2 as a
-// warp scan, 32 rows per step
-template <class FS> __global__ void __launch_bounds__(PA_THREADS) k_perm_apply(fe* z, const fe* __restrict__ tot, const fe* __restrict__ r,
-                                                                             size_t n, size_t last, const fe rand0, const fe rand1,
-                                                                             unsigned* final_is_one) {
-    if (blockIdx.x + 1 < gridDim.x) {
-        const size_t j = (size_t)blockIdx.x * PA_THREADS + threadIdx.x;
-        if (j > last) return;
-        fe v = load_fe(z + j);
-        const size_t b = j / PA_BLOCK_ROWS;
-        if (b) {
-            v = fe_mul<FS>(v, load_fe_nc(tot + b));
-            store_fe(z + j, v);
+    __device__ void operator()(fe* z, size_t last, unsigned lane) const {
+        if (lane == 0) {
+            store_fe(z + last + 1, rand0);
+            store_fe(z + last + 2, rand1);
         }
-        if (j == last) *final_is_one = fe_eq(v, fe_one<FS>()) ? 1u : 0u;
-        return;
-    }
-    if (threadIdx.x >= 32) return;
-    const unsigned lane = threadIdx.x;
-    if (lane == 0) {
-        store_fe(z + last + 1, rand0);
-        store_fe(z + last + 2, rand1);
-    }
-    fe carry = rand1;
-    for (size_t base = last + 2; base < n - 1; base += 32) {
-        const size_t j = base + lane;
-        fe v = j < n - 1 ? load_fe_nc(r + j) : fe_one<FS>();
+        fe carry = rand1;
+        for (size_t base = last + 2; base < n - 1; base += 32) {
+            const size_t j = base + lane;
+            fe v = j < n - 1 ? load_fe_nc(r + j) : fe_one<FS>();
 #pragma unroll
-        for (unsigned d = 1; d < 32; d <<= 1) {
-            const fe up = shfl_up_fe(v, d);
-            if (lane >= d) v = fe_mul<FS>(v, up);
+            for (unsigned d = 1; d < 32; d <<= 1) {
+                const fe up = shfl_up_fe(v, d);
+                if (lane >= d) v = fe_mul<FS>(v, up);
+            }
+            v = fe_mul<FS>(carry, v);
+            if (j < n - 1) store_fe(z + j + 1, v);
+            carry = shfl_fe(v, 31);
         }
-        v = fe_mul<FS>(carry, v);
-        if (j < n - 1) store_fe(z + j + 1, v);
-        carry = shfl_fe(v, 31);
     }
-}
+};
 
 template <class T>
 static int perm_aggreg_impl(zk_ctx* ctx, unsigned log_n, size_t zk_rows, const void* const d_w[7], const void* const d_sigma[7],
@@ -140,9 +77,9 @@ static int perm_aggreg_impl(zk_ctx* ctx, unsigned log_n, size_t zk_rows, const v
     using namespace host;
     using FS = typename T::Dev; using HP = typename T::Host;
     const size_t n = (size_t)1 << log_n, last = n - zk_rows;
-    PermAggArgs a{};
+    PermRows<FS> a{};
     for (int k = 0; k < 7; k++) { a.w[k] = (const fe*)d_w[k]; a.sigma[k] = (const fe*)d_sigma[k]; }
-    a.z = d_z; a.n = n; a.last = last; a.sigma_stride = sigma_stride;
+    a.sigma_stride = sigma_stride;
     hfe hb;
     memcpy(hb.l, beta, 32);
     memcpy(&a.beta, beta, 32);
@@ -153,9 +90,10 @@ static int perm_aggreg_impl(zk_ctx* ctx, unsigned log_n, size_t zk_rows, const v
         const hfe bs = mul<HP>(hb, s);
         memcpy(&a.bshift[k], bs.l, 32);
     }
-    fe r0, r1;
-    memcpy(&r0, rand, 32);
-    memcpy(&r1, rand + 4, 32);
+    PermTail<FS> tail{};
+    tail.n = n;
+    memcpy(&tail.rand0, rand, 32);
+    memcpy(&tail.rand1, rand + 4, 32);
 
     std::lock_guard<std::mutex> lk(ctx->mu);
     ZK_CUDA(cudaSetDevice(ctx->device));
@@ -165,33 +103,21 @@ static int perm_aggreg_impl(zk_ctx* ctx, unsigned log_n, size_t zk_rows, const v
     int rc = ctx_ntt_table_ptrs(ctx, T::id, log_n, false, &a.ulo, &a.mid, &a.hi2);
     if (rc) return rc;
     // context scratch: r over d1 | block totals | the final-value flag
-    const size_t blocks = (n + PA_BLOCK_ROWS - 1) / PA_BLOCK_ROWS;
     Layout lay;
-    const size_t o_r = lay.add(n * sizeof(fe)), o_tot = lay.add(blocks * sizeof(fe)), o_flag = lay.add(sizeof(unsigned));
+    const size_t o_r = lay.add(n * sizeof(fe)), o_tot = lay.add(agg_blocks(n) * sizeof(fe)), o_flag = lay.add(sizeof(unsigned));
     rc = ctx->d_perm.ensure(lay.total);
     if (rc) return rc;
-    a.r = ctx->d_perm.at<fe>(o_r);
-    a.block_tot = ctx->d_perm.at<fe>(o_tot);
+    fe* r = ctx->d_perm.at<fe>(o_r);
     unsigned* d_flag = ctx->d_perm.at<unsigned>(o_flag);
-    k_perm_ratios<FS><<<(unsigned)blocks, PA_THREADS, 0, st>>>(a);
-    ZK_CUDA(cudaGetLastError());
-    k_block_product_scan<FS, PA_THREADS><<<1, PA_THREADS, 0, st>>>(a.block_tot, blocks);
-    ZK_CUDA(cudaGetLastError());
-    k_perm_apply<FS><<<(unsigned)((last + PA_THREADS) / PA_THREADS + 1), PA_THREADS, 0, st>>>(d_z, a.block_tot, a.r, n, last, r0, r1, d_flag);
-    ZK_CUDA(cudaGetLastError());
-    ctx->launches += 3;
+    tail.r = r;
+    rc = agg_launch<FS>(ctx, a, tail, d_z, r, ctx->d_perm.at<fe>(o_tot), n, last, d_flag);
+    if (rc) return rc;
     rc = ctx_ntt_device(ctx, T::id, d_z, log_n, 1, 0, /* inverse = */ 1, /* coset = */ 0);     // Evaluations::interpolate
     if (rc) return rc;
-    ZK_CUDA(cudaMemcpyAsync(&pin->perm_final, d_flag, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    ZK_CUDA(cudaMemcpyAsync(&pin->agg_final, d_flag, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
     ZK_CUDA(cudaStreamSynchronize(st));
-    *final_is_one = pin->perm_final ? 1 : 0;
+    *final_is_one = pin->agg_final ? 1 : 0;
     return ZK_OK;
-}
-
-// [p, p + bytes) and [q, q + qbytes) share a byte
-static bool overlaps(const void* p, size_t bytes, const void* q, size_t qbytes) {
-    const uintptr_t a = (uintptr_t)p, b = (uintptr_t)q;
-    return a < b + qbytes && b < a + bytes;
 }
 
 }  // namespace zkb

@@ -23,7 +23,7 @@ struct PermQuotArgs {
     const fe* sigma[7]; // permutation_coefficients8
     const fe* z;
     const fe* zkpm;
-    const fe* ulo;      // x_i = omega_m^i from the forward transform's tables (ntt.cuh): ulo[i & 1023] * mid[(i >> 10) & 1023] * hi2[i >> 20]
+    const fe* ulo;      // x_i = omega_m^i from the forward transform's tables (domain_point, ntt.cuh)
     const fe* mid;
     const fe* hi2;
     fe* out;
@@ -36,10 +36,7 @@ struct PermQuotArgs {
 template <class FS> __global__ void __launch_bounds__(128) k_perm_quotient(const __grid_constant__ PermQuotArgs a) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= a.m) return;
-    fe x = load_fe_nc(a.ulo + (i & 1023));
-    if ((i >> 10) & 1023) x = fe_mul<FS>(x, load_fe_nc(a.mid + ((i >> 10) & 1023)));
-    if (i >> 20) x = fe_mul<FS>(x, load_fe_nc(a.hi2 + (i >> 20)));
-    const fe bx = fe_mul<FS>(a.beta, x);
+    const fe bx = fe_mul<FS>(a.beta, domain_point<FS>(a.ulo, a.mid, a.hi2, i));
     size_t inext = i + a.next_shift;
     if (inext >= a.m) inext -= a.m;
     fe shifts = load_fe_nc(a.z + i), sigmas = load_fe_nc(a.z + inext);

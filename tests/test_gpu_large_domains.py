@@ -230,7 +230,7 @@ def draw_scalars(P, seed):
 @pytest.mark.parametrize("fid,log_n,zk_rows,stride", [(0, 19, 3, 8), (1, 21, 9, 1)])
 def test_perm_aggreg_random_instance(ctx, orc, fid, log_n, zk_rows, stride):
     """random, unwired witness and sigma columns: z's coefficients and the final-value flag vs perm_replay.  At 2^19 the scan over
-    256 block totals gives each thread of k_perm_block_scan two of them; at 2^21 omega^j takes its third table factor past 2^20."""
+    256 block totals gives each thread of k_scan_block_totals two of them; at 2^21 omega^j takes its third table factor past 2^20."""
     P, n = orc.MODULUS[fid], 1 << log_n
     beta, gamma, shifts, rand = draw_scalars(P, 160 + log_n)
     w = orc.random_scalars(fid, 7 * n, seed=161).reshape(7, n, 4)

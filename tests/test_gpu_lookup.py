@@ -132,7 +132,9 @@ def test_joint_table(ctx, orc, fid, log_n, n_cols, ids, runtime):
 
 # ---------------------------------------------------------------------------------------------------------------- sorted + aggregation
 CASES = [(4, 3, 1, "first", 1), (4, 5, 3, "middle", 8), (4, 14, 4, "last", 8), (6, 62, 3, "end", 1), (10, 3, 4, "end", 8),
-         (10, 5, 1, "middle", 1), (12, 5, 4, "first", 8), (12, 3, 3, "last", 1), (16, 3, 4, "middle", 8), (17, 5, 4, "end", 8)]
+         (10, 5, 1, "middle", 1), (12, 5, 4, "first", 8), (12, 3, 3, "last", 1), (16, 3, 4, "middle", 8), (17, 5, 4, "end", 8),
+         # L + 1 = n - zk_rows just past, on and just before the 2048-row block boundary of the aggregation
+         (12, 2047, 2, "first", 8), (12, 2048, 4, "end", 1), (12, 2049, 3, "middle", 8)]
 
 
 @pytest.mark.parametrize("fid", [0, 1])

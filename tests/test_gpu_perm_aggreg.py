@@ -97,7 +97,9 @@ def variants(orc, fid, log_n, zk_rows, inst, rng):
     return out
 
 
-CASES = [(log_n, zk) for log_n in (4, 10, 16, 17) for zk in (3, 5, (1 << log_n) - 1)]
+# 2^12 rows: last = n - zk_rows just past, on and just before the 2048-row block boundary (2049, 2048, 2047), on a 16-row
+# thread boundary (16), and a tail warp scan over 31 or 32 rows (zk_rows 35, 36)
+CASES = [(log_n, zk) for log_n in (4, 10, 16, 17) for zk in (3, 5, (1 << log_n) - 1)] + [(12, zk) for zk in (35, 36, 2047, 2048, 2049, 4080)]
 
 
 @pytest.mark.parametrize("fid", [0, 1])
