@@ -14,6 +14,30 @@ pub struct zk_bases {
 pub struct zk_srs {
     _p: [u8; 0],
 }
+#[repr(C)]
+pub struct zk_index_cache {
+    _p: [u8; 0],
+}
+
+/// zk_index_header: the cache file's ScalarHeader and preamble fields (kimchi/src/cached_prover_index.rs:173-225)
+#[repr(C)]
+pub struct zk_index_header {
+    pub public_inputs: u32,
+    pub prev_challenges: u32,
+    pub zk_rows: u64,
+    pub max_poly_size: u64,
+    pub domain_d1_size: u64,
+    pub feature_flags: u32,
+    pub optional_selectors_present: u32,
+    pub lookup_selectors_present: u32,
+    pub num_sections: u32,
+    pub disable_gates_checks: c_int,
+    pub has_verifier_index_digest: c_int,
+    pub endo: [u64; 4],
+    pub shift: [[u64; 4]; 7],
+    pub verifier_index_digest: [u64; 4],
+    pub identifier: [c_char; 512],
+}
 
 pub const ZK_FP: c_int = 0;
 pub const ZK_FQ: c_int = 1;
@@ -210,4 +234,13 @@ extern "C" {
 
     pub fn zk_ntt_batch(ctx: *mut zk_ctx, field_id: c_int, data: *mut u64, log_n: c_uint, batch: usize, in_len: usize, inverse: c_int,
                         coset: c_int) -> c_int;
+
+    pub fn zk_index_cache_free(cache: *mut zk_index_cache);
+    pub fn zk_index_cache_header(cache: *const zk_index_cache, out: *mut zk_index_header) -> c_int;
+    pub fn zk_index_cache_section(cache: *const zk_index_cache, tag: u32, d_ptr: *mut *const c_void, n_elems: *mut usize,
+                                  elem_domain_size: *mut u32) -> c_int;
+    pub fn zk_index_build(ctx: *mut zk_ctx, field_id: c_int, hdr: *const zk_index_header, gates: *const c_void, n_gates: usize,
+                          gate_coeffs: *const c_void, gate_coeffs_len: usize, zero_selectors: c_int, out: *mut *mut zk_index_cache) -> c_int;
+    pub fn zk_index_commitments(srs: *mut zk_srs, index: *const zk_index_cache, out_xy: *mut u64, capacity_points: usize,
+                                out_points: *mut usize) -> c_int;
 }

@@ -15,6 +15,9 @@
 //!   and sigma_6 over d8, leaving ft resident for the opening proof (`zk_prover_ft_dev`).
 //! * [`perm::perm_aggreg_dev`] builds the permutation aggregation polynomial z (kimchi/src/circuits/polynomials/permutation.rs:447-574)
 //!   from the resident witness and `permutation_coefficients8`, leaving z resident (`zk_perm_aggreg_dev`).
+//! * [`index::DeviceIndex`] builds the prover index's column evaluations (kimchi/src/circuits/constraints.rs:510-760) on the device
+//!   from `cs.gates` and the commitments of its verifier index (kimchi/src/verifier_index.rs:221-300) (`zk_index_build`,
+//!   `zk_index_commitments`).
 //! * [`lookup::LookupLowering`] builds the lookup argument's joint table, sorted columns and aggregation polynomial
 //!   (kimchi/src/prover.rs:383-673) from the resident witness and the index cache's lookup tables (`zk_lookup_*_dev`).
 //!
@@ -25,6 +28,7 @@ pub mod evals;
 pub mod expr;
 pub mod ffi;
 pub mod ft;
+pub mod index;
 pub mod lookup;
 pub mod marshal;
 pub mod open;

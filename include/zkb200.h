@@ -519,6 +519,36 @@ void zk_index_cache_free(zk_index_cache* cache);
 int zk_index_cache_header(const zk_index_cache* cache, zk_index_header* out);
 int zk_index_cache_section(const zk_index_cache* cache, uint32_t tag, const void** d_ptr, size_t* n_elems, uint32_t* elem_domain_size);
 
+/* ------------------------------------------------------------------ prover index built on the device
+ * zk_index_build        ConstraintSystem::evaluated_column_coefficients + column_evaluations (kimchi/src/circuits/constraints.rs:510-760,
+ *                       selector_polynomial :334-362) from the circuit's gates, into a handle that zk_index_cache_section / _header / _free
+ *                       serve like a loaded file.  Inputs are the cache file's own encodings (cached_prover_index.rs:270-300, :965-1015,
+ *                       :1472-1479):
+ *   gates               n_gates PrunedGate records of 60 bytes: typ_tag u16 | pad[2] | 7 x (row u32, col u32); tags 0 .. 13
+ *   gate_coeffs         per gate a u32 count, then that many Montgomery field elements; exactly n_gates records
+ *   hdr                 domain_d1_size (n, a power of two <= 2^27), zk_rows (3 .. n - 1), shift[7] (Montgomery, canonical) and
+ *                       optional_selectors_present (bits 0 .. 5: RangeCheck0, RangeCheck1, ForeignFieldAdd, ForeignFieldMul, Xor16, Rot64)
+ *                       select the work; the other fields are copied into the handle's header, num_sections = the sections made
+ *   zero_selectors      the reference's `cfg!(debug_assertions) && disable_gates_checks`: selector_polynomial's sections are zero
+ * Rows n_gates .. n - 1 are CircuitGate::zero gates wired to themselves (constraints.rs:1010-1020).  Sections, Montgomery, with
+ * elem_domain_size 8n over d8 and 4n over d4: 0x01 sid (n, omega^j); 0x30 + k sigma_k over d8 (shift[col] omega^row of wire k, zero on
+ * rows n + 2 - zk_rows .. n - 2); 0x10 + i coefficients8[i] (coeffs[i], zero past a gate's count; i >= 15 ignored); 0x20 generic over
+ * d4; 0x21 poseidon over d8; 0x22 complete_add over d4; 0x23 VarBaseMul, 0x24 EndoMul, 0x25 EndoMulScalar over d8; 0x40 + b the optional
+ * selectors of the bits set.  Runs on the context's stream and synchronises once.  ZK_ERR_INVALID, *out = NULL, nothing published:
+ * a null pointer, an unknown field, a bad n or zk_rows, n_gates > n, a tag > 13, a wire with row >= n or col >= 7, gate_coeffs not
+ * exactly n_gates records, optional bits beyond bit 5, a shift or coefficient that is not a canonical field element.
+ * zk_index_commitments  the commitments of ProverIndex::verifier_index (kimchi/src/verifier_index.rs:221-300) for any index handle,
+ *                       built or loaded: commit_evaluations_non_hiding(d1, section) of sigma 0..6, coefficients 0..14, generic, psm,
+ *                       complete_add, mul, emul, endomul_scalar (these six masked with blinder one: every chunk + h, :179-185), then
+ *                       the present optional selectors in bit order.  Each has chunks = zk_srs_lagrange_basis_chunks(srs, n) affine
+ *                       points; out_xy receives them commitment-major, *out_points the total.  The d1 Lagrange basis is built if the
+ *                       SRS has none.  Only points cross PCIe.  ZK_ERR_INVALID: a null pointer, a built index of another field than
+ *                       the SRS's scalar field, a required section missing or not a multiple of n elements, a header bit whose section
+ *                       is missing, capacity_points too small. */
+int zk_index_build(zk_ctx* ctx, int field_id, const zk_index_header* hdr, const void* gates, size_t n_gates, const void* gate_coeffs,
+                   size_t gate_coeffs_len, int zero_selectors, zk_index_cache** out);
+int zk_index_commitments(zk_srs* srs, const zk_index_cache* index, uint64_t* out_xy, size_t capacity_points, size_t* out_points);
+
 /* ------------------------------------------------------------------ diagnostics (tests/test_gpu_field.py, DESIGN.md compute model)
  * Element-wise device field ops on n elements (op: 0 mul, 1 add, 2 sub, 3 inverse of a), host pointers. */
 int zk_debug_field_op(zk_ctx* ctx, int field_id, int op, const uint64_t* a, const uint64_t* b, uint64_t* out, size_t n);

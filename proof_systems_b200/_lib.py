@@ -118,6 +118,8 @@ def lib() -> ctypes.CDLL:
     L.zk_index_cache_free.restype = None
     L.zk_index_cache_header.argtypes = [vp, ctypes.POINTER(IndexHeader)]
     L.zk_index_cache_section.argtypes = [vp, ctypes.c_uint32, ctypes.POINTER(vp), ctypes.POINTER(sz), ctypes.POINTER(ctypes.c_uint32)]
+    L.zk_index_build.argtypes = [vp, i, ctypes.POINTER(IndexHeader), vp, sz, vp, sz, i, ctypes.POINTER(vp)]
+    L.zk_index_commitments.argtypes = [vp, vp, _u64p, sz, ctypes.POINTER(sz)]
     L.zk_comm_unique_id.argtypes = [vp]
     L.zk_comm_init_rank.argtypes = [vp, vp, i, i, ctypes.POINTER(vp)]
     L.zk_comm_destroy.argtypes = [vp]

@@ -60,6 +60,7 @@ struct PinnedSlots {
     fe ft_eval1;
     unsigned agg_final;         // zk_perm_aggreg_dev / zk_lookup_aggreg_dev: z[n - zk_rows] == 1 / agg[n - zk_rows - 1] == 1
     unsigned lookup_sorted[2];  // zk_lookup_sorted_dev: the smallest row with a missing value (all ones: none), columns formed
+    unsigned index_bad;         // zk_index_build: a gate coefficient is not a canonical field element
 };
 
 // [p, p + bytes) and [q, q + qbytes) share a byte
@@ -174,4 +175,15 @@ struct zk_srs {
     zk_bases* g = nullptr;              // resident generators
     uint64_t h[8];                      // blinding base
     std::map<size_t, zk_bases*> lagrange;  // domain size -> resident Lagrange basis (one chunk per element: domain <= |g|)
+};
+
+// a prover index resident on the device: loaded from a cache file (index_cache.cu) or built from the gates (index_build.cu)
+struct zk_index_cache {
+    zk_ctx* ctx = nullptr;
+    int field = -1;                   // scalar field of a built index; a loaded file does not record it (-1)
+    zk_index_header hdr{};
+    struct Section { uint32_t tag; uint64_t offset, length; uint32_t elem_domain_size; };
+    std::vector<Section> sections;
+    zkb::DevScratch payload;          // bytes [lo, hi) of the image (a loaded file) or every section back to back (lo = 0, built)
+    uint64_t lo = 0, hi = 0;
 };

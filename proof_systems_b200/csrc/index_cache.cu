@@ -45,15 +45,6 @@ bool is_field_section(uint32_t tag) {
 
 }  // namespace
 
-struct zk_index_cache {
-    zk_ctx* ctx = nullptr;
-    zk_index_header hdr{};
-    struct Section { uint32_t tag; uint64_t offset, length; uint32_t elem_domain_size; };
-    std::vector<Section> sections;
-    zkb::DevScratch payload;          // image bytes [lo, hi) as they lie in the file
-    uint64_t lo = 0, hi = 0;
-};
-
 extern "C" {
 
 int zk_index_cache_load(zk_ctx* ctx, const void* image, size_t image_len, const char* expect_identifier, zk_index_cache** out) {

@@ -139,6 +139,18 @@ class SRS:
     def commit_evaluations_custom(self, domain_size: int, evals, blinders) -> PolyComm:
         return self.mask_custom(self.commit_evaluations_non_hiding(domain_size, evals), blinders)
 
+    def index_commitments(self, index: "IndexCache") -> np.ndarray:
+        """zk_index_commitments: the commitments of ProverIndex::verifier_index (kimchi/src/verifier_index.rs:221-300) of a built or
+        loaded index, uint64 [count, chunks, 8] affine: sigma 0..6, coefficients 0..14, generic, psm, complete_add, mul, emul,
+        endomul_scalar (those six masked with blinder one), then the present optional selectors in bit order."""
+        n = index.header.domain_d1_size
+        chunks = self.lagrange_basis_chunks(n)
+        count = 7 + 15 + 6 + bin(index.header.optional_selectors_present).count("1")
+        out = np.zeros((count * chunks, 8), dtype=np.uint64)
+        k = ctypes.c_size_t()
+        check(lib().zk_index_commitments(self._h, index._h, out.ctypes.data_as(_u64p), out.shape[0], ctypes.byref(k)))
+        return out[: k.value].reshape(-1, chunks, 8)
+
 
 class IndexCache:
     """A cached prover index (kimchi/src/cached_prover_index.rs:26-56, "MINAPK01") resident on the device: zk_index_cache_load parses the
@@ -154,6 +166,25 @@ class IndexCache:
         hdr = IndexHeader()
         check(lib().zk_index_cache_header(self._h, ctypes.byref(hdr)))
         self.header = hdr
+
+    @classmethod
+    def build(cls, ctx: Context, fid: int, header, gates: bytes, gate_coeffs: bytes, zero_selectors: bool = False) -> "IndexCache":
+        """zk_index_build: the prover index's column evaluations (constraints.rs:510-760) built on the device from the circuit's gates
+        in the cache file's encodings — `gates` the PrunedGate records (60 bytes each), `gate_coeffs` the GateCoeffs records — and an
+        IndexHeader with domain_d1_size, zk_rows, shift and optional_selectors_present set.  zero_selectors: the reference's
+        `cfg!(debug_assertions) && disable_gates_checks`."""
+        from ._lib import IndexHeader
+        self = cls.__new__(cls)
+        self.ctx, self._image, self._h = ctx, None, ctypes.c_void_p()
+        g, c = bytes(gates), bytes(gate_coeffs)
+        if len(g) % 60:
+            raise ValueError("gates: a whole number of 60-byte PrunedGate records expected")
+        check(lib().zk_index_build(ctx._h, fid, ctypes.byref(header), g or None, len(g) // 60, c or None, len(c), int(zero_selectors),
+                                   ctypes.byref(self._h)))
+        hdr = IndexHeader()
+        check(lib().zk_index_cache_header(self._h, ctypes.byref(hdr)))
+        self.header = hdr
+        return self
 
     @classmethod
     def from_file(cls, ctx: Context, path: str, expect_identifier: str | None = None) -> "IndexCache":
