@@ -213,21 +213,30 @@ def make_tables(rng, P, n_rows):
     return rows[:n_rows]
 
 
-def instance(P, log_n, zk_rows, m, seed, dummy_at="end", jc=None, empty_frac=0.3, gates=None, hot=False, table=None):
+def max_joint_size(patterns):
+    """LookupInfo::max_joint_size (lookups.rs:211-214): the most entries of any joint lookup of the patterns"""
+    return max((len(entries) for pat in patterns for _, entries in pat), default=0)
+
+
+def instance(P, log_n, zk_rows, m, seed, dummy_at="end", jc=None, empty_frac=0.3, gates=None, hot=False, table=None, tic=None):
     """A valid instance: every lookup of rows < L hits the table.  The table has L rows: random rows of the XOR, range-check, two
     width-2 (Lookup-pattern) and synthetic tables, duplicates, and the dummy row (0, 0, 0) of id 0 placed at the start, the middle
     or the end (dummy_at: "first", "middle", "end" = zero padding at the end, "last" = exactly one dummy row, at L - 1).
     T1[L] = T1[L - 1] (kimchi pads past L with the dummy too) and random beyond.  gates: a gate list for by_row, else random gates
-    drawn from those whose patterns fit m.  hot: every lookup hits one table row.  table: the L table rows to use instead."""
+    drawn from those whose patterns fit m.  hot: every lookup hits one table row.  table: the L table rows to use instead.
+    tic: the table id combiner; None draws it at random, "kimchi" takes jc^max_joint_size of the instance's patterns as the
+    prover does (prover.rs:480-486) and as the lookup constraints assume, an int is used as given.  The other draws do not depend
+    on it."""
     rng = random.Random(seed)
     n = 1 << log_n
     L = n - zk_rows - 1
     assert L >= 1
     jc = rng.randrange(P) if jc is None else jc
-    tic = rng.randrange(P)
+    drawn_tic = rng.randrange(P)
     coeff = rng.randrange(2, P)
     names = [p for p, k in (("xor", 4), ("lookup", 3), ("range_check", 4), ("foreign_field_mul", 4)) if k <= m] + ["synthetic"]
     patterns = [kimchi_lookups(p) if p != "synthetic" else synthetic_lookups(coeff) for p in names]
+    tic = drawn_tic if tic is None else pow(jc, max_joint_size(patterns), P) if tic == "kimchi" else tic % P
     pidx = {p: k + 1 for k, p in enumerate(names)}
     n_real = L - 1 if dummy_at == "last" else L - max(1, L // 4)
     real = make_tables(rng, P, n_real)
