@@ -241,6 +241,22 @@ def _out(n):
     return np.empty(n, dtype=np.uint64)
 
 
+def _fe(a, k: int = 4) -> np.ndarray:
+    """a field element as contiguous uint64 [4] Montgomery limbs, or k limbs of k / 4 elements (shifts, rand)"""
+    return np.ascontiguousarray(a, dtype=np.uint64).reshape(k)
+
+
+def _dptr(p) -> ctypes.c_void_p:
+    """a device pointer argument: an integer address, or None / 0 for NULL"""
+    return ctypes.c_void_p(int(p) if p else None)
+
+
+def _dptrs(ptrs, n: int = 0):
+    """a void*[] of device pointers: n slots (7 or 15 columns), or with n = 0 one per pointer and at least one"""
+    ptrs = [int(p) for p in ptrs]
+    return (ctypes.c_void_p * (n or max(1, len(ptrs))))(*ptrs)
+
+
 def jacobian_to_affine(curve: int, xyz) -> np.ndarray:
     """Projective::into_affine()"""
     xyz = np.ascontiguousarray(xyz, dtype=np.uint64)
@@ -256,7 +272,35 @@ def jacobian_sum(curve: int, pts) -> np.ndarray:
     return out
 
 
-class Context:
+class Handle:
+    """Something the library hands out and takes back: `_h` is what `_release` gives back, `ctx` the owning Context (None for a
+    Context itself).  close() releases it once and is harmless to repeat; a child whose Context is already closed is dropped
+    without a library call, since the Context took its resources with it.  Also a context manager, and closed when collected."""
+    _h = None
+    ctx = None
+
+    def _release(self, h):
+        raise NotImplementedError
+
+    def close(self):
+        h, self._h = self._h, None
+        if h and (self.ctx is None or self.ctx._h):
+            self._release(h)
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class Context(Handle):
     """One CUDA device (one per process/rank)."""
 
     def __init__(self, device: int = 0):
@@ -264,16 +308,12 @@ class Context:
         check(lib().zk_ctx_create(device, ctypes.byref(self._h)))
         self.device = device
 
-    def close(self):
-        if getattr(self, "_h", None):
-            lib().zk_ctx_destroy(self._h)
-            self._h = None
+    def _release(self, h):
+        lib().zk_ctx_destroy(h)
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+    def buffers(self) -> "DeviceBuffers":
+        """`with ctx.buffers() as bufs:` — device buffers freed together when the block ends, however it ends"""
+        return DeviceBuffers(self)
 
     def set_stream(self, cuda_stream: int | None):
         """None: the library's own stream.  An integer is a cudaStream_t handle, 0 included: 0 is the legacy default stream (torch's
@@ -372,12 +412,7 @@ class Context:
     def ntt(self, field: int, data, inverse: bool = False, coset: bool = False, in_len: int = 0) -> np.ndarray:
         """Transforms a copy.  data [n,4] or [batch,n,4] (Montgomery); n a power of two."""
         a = np.array(data, dtype=np.uint64, order="C", copy=True)
-        assert a.shape[-1] == 4
-        n = a.shape[-2]
-        batch = 1 if a.ndim == 2 else a.shape[0]
-        log_n = n.bit_length() - 1
-        assert 1 << log_n == n
-        check(lib().zk_ntt_batch(self._h, field, _ptr(a), log_n, batch, in_len, int(inverse), int(coset)))
+        self.ntt_inplace(field, a, inverse, coset, in_len)
         return a
 
     def ntt_inplace(self, field: int, a: np.ndarray, inverse: bool = False, coset: bool = False, in_len: int = 0):
@@ -419,12 +454,9 @@ class Context:
     def perm_quotient_dev(self, field: int, log_m: int, d_w, d_z: int, d_sigma, d_zkpm: int, beta, gamma, alpha0, shifts, d_out: int, next_shift: int = 8):
         """zk_perm_quotient_dev: the permutation part of the quotient over d8, operands resident on the device; d_w, d_sigma: 7 device
         pointers each"""
-        c = lambda a, k: np.ascontiguousarray(a, dtype=np.uint64).reshape(k)
-        b, g, a0, sh = c(beta, 4), c(gamma, 4), c(alpha0, 4), c(shifts, 28)
-        pw = (ctypes.c_void_p * 7)(*[int(p) for p in d_w])
-        ps = (ctypes.c_void_p * 7)(*[int(p) for p in d_sigma])
-        check(lib().zk_perm_quotient_dev(self._h, field, log_m, pw, ctypes.c_void_p(d_z), ps, ctypes.c_void_p(d_zkpm), _ptr(b), _ptr(g), _ptr(a0), _ptr(sh),
-                                         next_shift, ctypes.c_void_p(d_out)))
+        b, g, a0, sh = _fe(beta), _fe(gamma), _fe(alpha0), _fe(shifts, 28)
+        check(lib().zk_perm_quotient_dev(self._h, field, log_m, _dptrs(d_w, 7), _dptr(d_z), _dptrs(d_sigma, 7), _dptr(d_zkpm), _ptr(b), _ptr(g), _ptr(a0),
+                                         _ptr(sh), next_shift, _dptr(d_out)))
 
     def expr_eval_dev(self, field: int, tokens, constants, cols, out_len: int, out_domain_mult: int, d_out: int, accumulate: bool = False):
         """zk_expr_eval_dev: tokens = [(op, arg)], constants [k, 4] Montgomery, cols = [(device pointer, len, domain_mult)]"""
@@ -432,16 +464,16 @@ class Context:
         cn = np.ascontiguousarray(constants, dtype=np.uint64).reshape(-1, 4)
         cl = (ExprColumn * max(1, len(cols)))(*[ExprColumn(int(p), int(n), int(m), 0) for p, n, m in cols])
         check(lib().zk_expr_eval_dev(self._h, field, tk, len(tokens), _ptr(cn) if cn.size else None, cn.shape[0], cl, len(cols), out_len, out_domain_mult,
-                                     int(accumulate), ctypes.c_void_p(d_out)))
+                                     int(accumulate), _dptr(d_out)))
 
     def poly_add_dev(self, field: int, d_dst: int, d_src: int, length: int):
         """zk_poly_add_dev: dst[i] += src[i] on device-resident coefficient vectors"""
-        check(lib().zk_poly_add_dev(self._h, field, ctypes.c_void_p(d_dst), ctypes.c_void_p(d_src), length))
+        check(lib().zk_poly_add_dev(self._h, field, _dptr(d_dst), _dptr(d_src), length))
 
     def poly_divide_by_vanishing_dev(self, field: int, d_f: int, length: int, log_n: int, d_quot: int) -> bool:
         """zk_poly_divide_by_vanishing_dev: quotient of f by x^n - 1 into d_quot; returns whether the remainder is zero"""
         ok = ctypes.c_int()
-        check(lib().zk_poly_divide_by_vanishing_dev(self._h, field, ctypes.c_void_p(d_f), length, log_n, ctypes.c_void_p(d_quot), ctypes.byref(ok)))
+        check(lib().zk_poly_divide_by_vanishing_dev(self._h, field, _dptr(d_f), length, log_n, _dptr(d_quot), ctypes.byref(ok)))
         return bool(ok.value)
 
     # ------------------------------------------------------------------ evaluations at zeta / zeta*omega (zk_lagrange_*, zk_poly_evaluate_chunks_dev)
@@ -453,17 +485,16 @@ class Context:
     def lagrange_basis_evals_dev(self, field: int, log_n: int, max_poly_size: int, x, d_out: int) -> int:
         """zk_lagrange_evals_dev: LagrangeBasisEvaluations::new(max_poly_size, D(2^log_n), x) into d_out (chunks x 2^log_n elements,
         chunk-major); returns the chunk count"""
-        xv = np.ascontiguousarray(x, dtype=np.uint64).reshape(4)
-        check(lib().zk_lagrange_evals_dev(self._h, field, log_n, max_poly_size, _ptr(xv), ctypes.c_void_p(d_out)))
+        xv = _fe(x)
+        check(lib().zk_lagrange_evals_dev(self._h, field, log_n, max_poly_size, _ptr(xv), _dptr(d_out)))
         return self.lagrange_evals_chunks(1 << log_n, max_poly_size)
 
     def lagrange_evaluate_dev(self, field: int, d_bases, log_n: int, chunks: int, columns) -> np.ndarray:
         """zk_lagrange_evaluate_dev: columns = [(device pointer, len, boolean)] against the bases d_bases (one device pointer per point,
         built with the same log_n and chunks) -> uint64 [n_cols, n_points, chunks, 4] Montgomery"""
-        bases = (ctypes.c_void_p * max(1, len(d_bases)))(*[int(p) for p in d_bases])
         cols = (EvalColumn * max(1, len(columns)))(*[EvalColumn(int(p), int(n), int(bool(b)), 0) for p, n, b in columns])
         out = np.zeros((len(columns), len(d_bases), chunks, 4), dtype=np.uint64)
-        check(lib().zk_lagrange_evaluate_dev(self._h, field, bases, len(d_bases), log_n, chunks, cols, len(columns), _ptr(out)))
+        check(lib().zk_lagrange_evaluate_dev(self._h, field, _dptrs(d_bases), len(d_bases), log_n, chunks, cols, len(columns), _ptr(out)))
         return out
 
     def poly_evaluate_chunks_dev(self, field: int, polys, num_chunks: int, chunk_size: int, points) -> np.ndarray:
@@ -482,14 +513,14 @@ class Context:
         terms = [(device pointer, len, coeff_mont)], ft = f's chunks linearised at zeta^m minus (zeta^n - 1) times t's (d_t: t_len
         resident coefficients), written to d_ft (room for max_poly_size elements, zero past ft_len).  Returns (ft_len, ft(zeta omega)
         as uint64 [4] Montgomery)."""
-        zv = np.ascontiguousarray(zeta_mont, dtype=np.uint64).reshape(4)
+        zv = _fe(zeta_mont)
         arr = (LinTerm * max(1, len(terms)))()
         for k, (p, n, c) in enumerate(terms):
             arr[k].d_evals, arr[k].len = int(p), int(n)
-            arr[k].coeff[:] = [int(v) for v in np.ascontiguousarray(c, dtype=np.uint64).reshape(4)]
+            arr[k].coeff[:] = [int(v) for v in _fe(c)]
         ft_len, ev1 = ctypes.c_size_t(), np.zeros(4, dtype=np.uint64)
-        check(lib().zk_prover_ft_dev(self._h, field, log_n, max_poly_size, arr, len(terms), ctypes.c_void_p(d_t), t_len, _ptr(zv),
-                                     ctypes.c_void_p(d_ft), ctypes.byref(ft_len), _ptr(ev1)))
+        check(lib().zk_prover_ft_dev(self._h, field, log_n, max_poly_size, arr, len(terms), _dptr(d_t), t_len, _ptr(zv), _dptr(d_ft),
+                                     ctypes.byref(ft_len), _ptr(ev1)))
         return int(ft_len.value), ev1
 
     # ------------------------------------------------------------------ permutation aggregation polynomial z (zk_perm_aggreg_dev)
@@ -498,13 +529,10 @@ class Context:
         d_w (2^log_n evaluations each) and the 7 resident sigma columns d_sigma (sigma_len evaluations each, read at stride
         sigma_len / 2^log_n); beta, gamma [4], shifts [7, 4] and rand [2, 4] (the two F::rand draws) Montgomery.  Returns whether
         z[n - zk_rows] == 1 (the reference's "final value" check); z is written either way."""
-        c = lambda a, k: np.ascontiguousarray(a, dtype=np.uint64).reshape(k)
-        b, g, sh, rn = c(beta, 4), c(gamma, 4), c(shifts, 28), c(rand, 8)
-        pw = (ctypes.c_void_p * 7)(*[int(p) for p in d_w])
-        ps = (ctypes.c_void_p * 7)(*[int(p) for p in d_sigma])
+        b, g, sh, rn = _fe(beta), _fe(gamma), _fe(shifts, 28), _fe(rand, 8)
         ok = ctypes.c_int()
-        check(lib().zk_perm_aggreg_dev(self._h, field, log_n, zk_rows, pw, ps, sigma_len, _ptr(b), _ptr(g), _ptr(sh), _ptr(rn),
-                                       ctypes.c_void_p(d_z), ctypes.byref(ok)))
+        check(lib().zk_perm_aggreg_dev(self._h, field, log_n, zk_rows, _dptrs(d_w, 7), _dptrs(d_sigma, 7), sigma_len, _ptr(b), _ptr(g), _ptr(sh),
+                                       _ptr(rn), _dptr(d_z), ctypes.byref(ok)))
         return bool(ok.value)
 
     # ------------------------------------------------------------------ lookup argument (zk_lookup_*_dev)
@@ -513,11 +541,9 @@ class Context:
         """zk_lookup_joint_table_dev: T8[i] = sum_c jc^c col_c[i] + tic tid8[i] over d8 from the resident columns d_cols (8 * 2^log_n
         evaluations each; d_runtime8 is added to column 1), into d_out8 and, if given, its d1 values into d_out1.  Queued on the
         context's stream."""
-        c = lambda a: np.ascontiguousarray(a, dtype=np.uint64).reshape(4)
-        jc, tic = c(joint_combiner), c(table_id_combiner)
-        cols = (ctypes.c_void_p * max(1, len(d_cols)))(*[int(p) for p in d_cols])
-        check(lib().zk_lookup_joint_table_dev(self._h, field, log_n, cols, len(d_cols), ctypes.c_void_p(d_table_ids8), ctypes.c_void_p(d_runtime8),
-                                              _ptr(jc), _ptr(tic), ctypes.c_void_p(d_out8), ctypes.c_void_p(d_out1)))
+        jc, tic = _fe(joint_combiner), _fe(table_id_combiner)
+        check(lib().zk_lookup_joint_table_dev(self._h, field, log_n, _dptrs(d_cols), len(d_cols), _dptr(d_table_ids8), _dptr(d_runtime8), _ptr(jc),
+                                              _ptr(tic), _dptr(d_out8), _dptr(d_out1)))
 
     def lookup_sorted_dev(self, field: int, log_n: int, zk_rows: int, d_w, d_table: int, table_stride: int, info, rand, d_sorted) -> int:
         """zk_lookup_sorted_dev (lookup::constraints::sorted + zk_patch): the max_per_row + 1 sorted columns (d1 evaluations) into
@@ -525,31 +551,26 @@ class Context:
         structure (host.LookupSpec.info); rand: [(m + 1) * zk_rows, 4] Montgomery, column by column.  Returns -1, or the smallest row
         whose lookup value is not in the table (ValueNotInTable; d_sorted is then untouched)."""
         rn = np.ascontiguousarray(rand, dtype=np.uint64).reshape(-1)
-        pw = (ctypes.c_void_p * 15)(*[int(p) for p in d_w])
-        ps = (ctypes.c_void_p * max(1, len(d_sorted)))(*[int(p) for p in d_sorted])
         row = ctypes.c_int64(-2)
-        check(lib().zk_lookup_sorted_dev(self._h, field, log_n, zk_rows, pw, ctypes.c_void_p(d_table), table_stride, ctypes.byref(info),
-                                         _ptr(rn) if rn.size else None, ps, ctypes.byref(row)))
+        check(lib().zk_lookup_sorted_dev(self._h, field, log_n, zk_rows, _dptrs(d_w, 15), _dptr(d_table), table_stride, ctypes.byref(info),
+                                         _ptr(rn) if rn.size else None, _dptrs(d_sorted), ctypes.byref(row)))
         return int(row.value)
 
     def lookup_aggreg_dev(self, field: int, log_n: int, zk_rows: int, d_w, d_table: int, table_stride: int, info, d_sorted, beta, gamma, rand,
                           d_aggreg: int) -> bool:
         """zk_lookup_aggreg_dev (lookup::constraints::aggregation): the lookup aggregation polynomial's 2^log_n d1 evaluations into
         d_aggreg; rand: [zk_rows, 4] Montgomery.  Returns whether agg[n - zk_rows - 1] == 1 (the reference's debug assertion)."""
-        c = lambda a: np.ascontiguousarray(a, dtype=np.uint64).reshape(4)
-        b, g = c(beta), c(gamma)
+        b, g = _fe(beta), _fe(gamma)
         rn = np.ascontiguousarray(rand, dtype=np.uint64).reshape(-1)
-        pw = (ctypes.c_void_p * 15)(*[int(p) for p in d_w])
-        ps = (ctypes.c_void_p * max(1, len(d_sorted)))(*[int(p) for p in d_sorted])
         ok = ctypes.c_int()
-        check(lib().zk_lookup_aggreg_dev(self._h, field, log_n, zk_rows, pw, ctypes.c_void_p(d_table), table_stride, ctypes.byref(info), ps,
-                                         _ptr(b), _ptr(g), _ptr(rn) if rn.size else None, ctypes.c_void_p(d_aggreg), ctypes.byref(ok)))
+        check(lib().zk_lookup_aggreg_dev(self._h, field, log_n, zk_rows, _dptrs(d_w, 15), _dptr(d_table), table_stride, ctypes.byref(info),
+                                         _dptrs(d_sorted), _ptr(b), _ptr(g), _ptr(rn) if rn.size else None, _dptr(d_aggreg), ctypes.byref(ok)))
         return bool(ok.value)
 
     def points_fold_dev(self, curve: int, d_g: int, h: int, u_mont, d_out: int):
         """zk_points_fold_dev: out[i] = g[i] + [u] g[h + i] on device-resident affine points (the reference's per-round base fold)"""
-        u = np.ascontiguousarray(u_mont, dtype=np.uint64).reshape(4)
-        check(lib().zk_points_fold_dev(self._h, curve, ctypes.c_void_p(d_g), h, _ptr(u), ctypes.c_void_p(d_out)))
+        u = _fe(u_mont)
+        check(lib().zk_points_fold_dev(self._h, curve, _dptr(d_g), h, _ptr(u), _dptr(d_out)))
 
     # ------------------------------------------------------------------ diagnostics
     def field_op(self, field: int, op: str, a, b=None) -> np.ndarray:
@@ -571,7 +592,32 @@ class Context:
         return v.value
 
 
-class Bases:
+class DeviceBuffers(Handle):
+    """Device buffers owned together (Context.buffers()): close() frees each pointer put() or alloc() returned once, through
+    dev_free, which synchronises the stream first, so no queued work can still read a freed buffer."""
+
+    def __init__(self, ctx: Context):
+        self.ctx, self._h = ctx, []
+
+    def _release(self, ptrs):
+        for p in ptrs:
+            self.ctx.dev_free(p)
+
+    def alloc(self, nbytes: int) -> int:
+        p = self.ctx.dev_alloc(nbytes)
+        self._h.append(p)
+        return p
+
+    def put(self, a) -> int:
+        """a copy of the uint64 array a on the device; an empty array still gets 32 bytes, since the library refuses NULL"""
+        a = np.ascontiguousarray(a, dtype=np.uint64)
+        p = self.alloc(max(a.nbytes, 32))
+        if a.nbytes:
+            self.ctx.dev_upload(p, a)
+        return p
+
+
+class Bases(Handle):
     """Resident MSM bases (SRS::g or one Lagrange basis) on the context's device."""
 
     def __init__(self, ctx: Context, curve: int, points, window_bits: int = -1, device_ptr: int | None = None, n: int | None = None):
@@ -590,14 +636,7 @@ class Bases:
     def window_bits(self) -> int:
         return int(lib().zk_bases_window_bits(self._h))
 
-    def free(self):
-        if getattr(self, "_h", None):
-            lib().zk_bases_free(self._h)
-            self._h = None
+    def _release(self, h):
+        lib().zk_bases_free(h)
 
-    def __del__(self):
-        try:
-            if self.ctx._h:
-                self.free()
-        except Exception:
-            pass
+    free = Handle.close

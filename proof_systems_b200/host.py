@@ -13,7 +13,8 @@ from dataclasses import dataclass
 
 import numpy as np
 
-from ._lib import BASE_FIELD, FP, FQ, SCALAR_FIELD, Context, ZkError, _np_u64, _ptr, _u64p, check, lib
+from ._lib import (BASE_FIELD, FINAL_CB, FP, FQ, ROUND_CB, SCALAR_FIELD, U_BASE_CB, Context, Handle, IndexHeader, LookupInfo, LookupJoint,
+                   LookupTerm, OpenPoly, OpenTranscript, VerifyProof, ZkError, _fe, _np_u64, _ptr, _u64p, check, jacobian_to_affine, lib)
 
 
 class BlindersDontMatch(ValueError):
@@ -29,13 +30,13 @@ class PolyComm:
         return self.chunks.shape[0]
 
 
-class SRS:
+class SRS(Handle):
     """ipa::SRS<G>{g, h, lagrange_bases} with g (and every registered Lagrange basis) resident on the device."""
 
     def __init__(self, ctx: Context, curve: int, g, h, window_bits: int = -1):
         self.ctx, self.curve = ctx, curve
         self.g = _np_u64(g, (8,))
-        self.h = np.ascontiguousarray(h, dtype=np.uint64).reshape(8)
+        self.h = _fe(h, 8)
         self._h = ctypes.c_void_p()
         check(lib().zk_srs_create(ctx._h, curve, _ptr(self.g), self.g.shape[0], self.h.ctypes.data_as(_u64p), window_bits, ctypes.byref(self._h)))
 
@@ -53,17 +54,8 @@ class SRS:
                     srs.add_lagrange_basis(n, ctx.points_from_uncompressed(curve, basis[:, 0]))
         return srs
 
-    def close(self):
-        if getattr(self, "_h", None):
-            lib().zk_srs_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            if self.ctx._h:
-                self.close()
-        except Exception:
-            pass
+    def _release(self, h):
+        lib().zk_srs_destroy(h)
 
     # fn max_poly_size(&self) -> usize  /  fn size(&self)
     def max_poly_size(self) -> int:
@@ -152,20 +144,20 @@ class SRS:
         return out[: k.value].reshape(-1, chunks, 8)
 
 
-class IndexCache:
+class IndexCache(Handle):
     """A cached prover index (kimchi/src/cached_prover_index.rs:26-56, "MINAPK01") resident on the device: zk_index_cache_load parses the
     header and the section table and copies the payload as it lies in the file — raw Montgomery limbs are the device format."""
 
-    def __init__(self, ctx: Context, image: bytes, expect_identifier: str | None = None):
-        from ._lib import IndexHeader
-        self.ctx = ctx
-        self._image = np.frombuffer(image, dtype=np.uint8)          # keeps the bytes alive during the copy
-        self._h = ctypes.c_void_p()
-        ident = expect_identifier.encode() if expect_identifier is not None else None
-        check(lib().zk_index_cache_load(ctx._h, ctypes.c_void_p(self._image.ctypes.data), self._image.size, ident, ctypes.byref(self._h)))
-        hdr = IndexHeader()
-        check(lib().zk_index_cache_header(self._h, ctypes.byref(hdr)))
-        self.header = hdr
+    def __init__(self, ctx: Context, image: bytes | None = None, expect_identifier: str | None = None, _create=None):
+        """_create(out): the library call that writes the handle (IndexCache.build); by default zk_index_cache_load of image"""
+        if _create is None:
+            buf = np.frombuffer(image, dtype=np.uint8)
+            ident = expect_identifier.encode() if expect_identifier is not None else None
+            _create = lambda out: lib().zk_index_cache_load(ctx._h, ctypes.c_void_p(buf.ctypes.data), buf.size, ident, out)
+        self.ctx, self._h = ctx, ctypes.c_void_p()
+        check(_create(ctypes.byref(self._h)))
+        self.header = IndexHeader()
+        check(lib().zk_index_cache_header(self._h, ctypes.byref(self.header)))
 
     @classmethod
     def build(cls, ctx: Context, fid: int, header, gates: bytes, gate_coeffs: bytes, zero_selectors: bool = False) -> "IndexCache":
@@ -173,18 +165,11 @@ class IndexCache:
         in the cache file's encodings — `gates` the PrunedGate records (60 bytes each), `gate_coeffs` the GateCoeffs records — and an
         IndexHeader with domain_d1_size, zk_rows, shift and optional_selectors_present set.  zero_selectors: the reference's
         `cfg!(debug_assertions) && disable_gates_checks`."""
-        from ._lib import IndexHeader
-        self = cls.__new__(cls)
-        self.ctx, self._image, self._h = ctx, None, ctypes.c_void_p()
         g, c = bytes(gates), bytes(gate_coeffs)
         if len(g) % 60:
             raise ValueError("gates: a whole number of 60-byte PrunedGate records expected")
-        check(lib().zk_index_build(ctx._h, fid, ctypes.byref(header), g or None, len(g) // 60, c or None, len(c), int(zero_selectors),
-                                   ctypes.byref(self._h)))
-        hdr = IndexHeader()
-        check(lib().zk_index_cache_header(self._h, ctypes.byref(hdr)))
-        self.header = hdr
-        return self
+        return cls(ctx, _create=lambda out: lib().zk_index_build(ctx._h, fid, ctypes.byref(header), g or None, len(g) // 60, c or None, len(c),
+                                                                int(zero_selectors), out))
 
     @classmethod
     def from_file(cls, ctx: Context, path: str, expect_identifier: str | None = None) -> "IndexCache":
@@ -199,17 +184,8 @@ class IndexCache:
         check(lib().zk_index_cache_section(self._h, tag, ctypes.byref(p), ctypes.byref(n), ctypes.byref(d)))
         return p.value or 0, n.value, d.value
 
-    def close(self):
-        if getattr(self, "_h", None):
-            lib().zk_index_cache_free(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            if self.ctx._h:
-                self.close()
-        except Exception:
-            pass
+    def _release(self, h):
+        lib().zk_index_cache_free(h)
 
 
 class OpeningProof:
@@ -220,12 +196,47 @@ class OpeningProof:
         self.lr, self.delta, self.z1, self.z2, self.sg = lr, delta, z1, z2, sg
 
 
+class _Transcript:
+    """The caller's transcript callables u_base(cip [4]) -> U [8], round_challenge(i, l [8], r [8]) -> u [4] and
+    final_challenge(delta [8]) -> c [4] as a zk_open_transcript (`struct`).  An exception never unwinds through the C frames: the
+    first one is kept, the callback returns 1 so that the library fails the call, and reraise() raises it once the call is back."""
+
+    def __init__(self, u_base, round_challenge, final_challenge):
+        self.error = None
+        self.callbacks = (U_BASE_CB(self.guard(lambda cip, out: _put(out, u_base(_view(cip, 4)), 8))),
+                          ROUND_CB(self.guard(lambda i, l, r, out: _put(out, round_challenge(int(i), _view(l, 8), _view(r, 8)), 4))),
+                          FINAL_CB(self.guard(lambda d, out: _put(out, final_challenge(_view(d, 8)), 4))))
+        self.struct = OpenTranscript(None, *self.callbacks)
+
+    def guard(self, fn):
+        def wrapped(user, *args):
+            try:
+                fn(*args)
+                return 0
+            except Exception as e:
+                if self.error is None:
+                    self.error = e
+                return 1
+        return wrapped
+
+    def reraise(self):
+        if self.error is not None:
+            raise self.error
+
+
+def _view(p, n):
+    return np.ctypeslib.as_array(p, shape=(n,)).copy()
+
+
+def _put(p, v, n):
+    np.ctypeslib.as_array(p, shape=(n,))[:] = np.ascontiguousarray(v, dtype=np.uint64).reshape(n)
+
+
 def srs_open(srs, plnms, elm, polyscale, evalscale, rng_scalars, u_base, round_challenge, final_challenge) -> OpeningProof:
     """SRS::open (ipa.rs:823-1061) through zk_srs_open.
     plnms: list of (data [len, 4] Montgomery numpy array OR (device_ptr, len), domain_size (0 = coefficients), blinders [k, 4]);
     elm [m, 4]; rng_scalars [2 * rounds + 2, 4] = rand_l, rand_r per round, then d, r_delta; the three callables are the caller's
     transcript: u_base(cip [4]) -> U [8]; round_challenge(i, l [8], r [8]) -> u [4]; final_challenge(delta [8]) -> c [4]."""
-    from ._lib import FINAL_CB, ROUND_CB, U_BASE_CB, OpenPoly, OpenTranscript
     keep, arr = [], (OpenPoly * max(1, len(plnms)))()
     for i, (data, dom, blinders) in enumerate(plnms):
         if isinstance(data, tuple):
@@ -239,39 +250,16 @@ def srs_open(srs, plnms, elm, polyscale, evalscale, rng_scalars, u_base, round_c
         arr[i] = OpenPoly(ptr, ln, dom, bl.ctypes.data, bl.shape[0])
     elm = _np_u64(elm, (4,))
     rng = _np_u64(rng_scalars, (4,))
-    ps = np.ascontiguousarray(polyscale, dtype=np.uint64).reshape(4)
-    es = np.ascontiguousarray(evalscale, dtype=np.uint64).reshape(4)
-    errors = []
-
-    def view(p, n):
-        return np.ctypeslib.as_array(p, shape=(n,)).copy()
-
-    def put(p, v, n):
-        np.ctypeslib.as_array(p, shape=(n,))[:] = np.ascontiguousarray(v, dtype=np.uint64).reshape(n)
-
-    def guard(fn):
-        def wrapped(*a):
-            try:
-                fn(*a)
-                return 0
-            except Exception as e:           # never unwind through the C frames
-                errors.append(e)
-                return 1
-        return wrapped
-
-    cb_u = U_BASE_CB(guard(lambda user, cip, out: put(out, u_base(view(cip, 4)), 8)))
-    cb_r = ROUND_CB(guard(lambda user, i, l, r, out: put(out, round_challenge(int(i), view(l, 8), view(r, 8)), 4)))
-    cb_f = FINAL_CB(guard(lambda user, d, out: put(out, final_challenge(view(d, 8)), 4)))
-    tr = OpenTranscript(None, cb_u, cb_r, cb_f)
+    ps, es = _fe(polyscale), _fe(evalscale)
+    tr = _Transcript(u_base, round_challenge, final_challenge)
     rounds_cap = 64
     lr = np.zeros((rounds_cap, 2, 8), dtype=np.uint64)
     delta, sg = np.zeros(8, dtype=np.uint64), np.zeros(8, dtype=np.uint64)
     z1, z2 = np.zeros(4, dtype=np.uint64), np.zeros(4, dtype=np.uint64)
     rounds = ctypes.c_size_t(0)
-    rc = lib().zk_srs_open(srs._h, arr, len(plnms), _ptr(elm), elm.shape[0], _ptr(ps), _ptr(es), _ptr(rng), rng.shape[0], ctypes.byref(tr),
+    rc = lib().zk_srs_open(srs._h, arr, len(plnms), _ptr(elm), elm.shape[0], _ptr(ps), _ptr(es), _ptr(rng), rng.shape[0], ctypes.byref(tr.struct),
                            _ptr(lr), rounds_cap, ctypes.byref(rounds), _ptr(delta), _ptr(z1), _ptr(z2), _ptr(sg))
-    if errors:
-        raise errors[0]
+    tr.reraise()
     check(rc)
     return OpeningProof(lr[: rounds.value].copy(), delta, z1, z2, sg)
 
@@ -297,24 +285,7 @@ def srs_verify(srs, batch, rand_base, sg_rand_base, return_sum: bool = False):
     """SRS::verify (ipa.rs:301-502) through zk_srs_verify: True iff the batch of BatchEvaluationProof verifies.  rand_base and
     sg_rand_base are the two scalars the reference draws from its rng (Montgomery [4]).  With return_sum, also the affine point [8]
     the reference compares with zero.  An exception raised by a callback aborts the call and is re-raised here."""
-    from ._lib import FINAL_CB, ROUND_CB, U_BASE_CB, OpenTranscript, VerifyProof
-    errors, keep = [], []
-
-    def view(p, n):
-        return np.ctypeslib.as_array(p, shape=(n,)).copy()
-
-    def put(p, v, n):
-        np.ctypeslib.as_array(p, shape=(n,))[:] = np.ascontiguousarray(v, dtype=np.uint64).reshape(n)
-
-    def guard(fn):
-        def wrapped(*a):
-            try:
-                fn(*a)
-                return 0
-            except Exception as e:           # never unwind through the C frames
-                errors.append(e)
-                return 1
-        return wrapped
+    keep, transcripts = [], []
 
     def arr(a, tail):
         a = _np_u64(a, tail) if np.size(a) else np.zeros((0,) + tail, dtype=np.uint64)
@@ -330,28 +301,25 @@ def srs_verify(srs, batch, rand_base, sg_rand_base, return_sum: bool = False):
         comms = [arr(c, (8,)) for c in e.commitments]
         cxy = arr(np.concatenate(comms) if comms else np.zeros((0, 8), dtype=np.uint64), (8,))
         chunks = (ctypes.c_size_t * max(1, len(comms)))(*[c.shape[0] for c in comms])
-        cb = (U_BASE_CB(guard(lambda user, c, out, f=e.u_base: put(out, f(view(c, 4)), 8))),
-              ROUND_CB(guard(lambda user, j, l, r, out, f=e.round_challenge: put(out, f(int(j), view(l, 8), view(r, 8)), 4))),
-              FINAL_CB(guard(lambda user, d, out, f=e.final_challenge: put(out, f(view(d, 8)), 4))))
-        tr = OpenTranscript(None, *cb)
-        keep += [chunks, cb, tr]
+        tr = _Transcript(e.u_base, e.round_challenge, e.final_challenge)
+        transcripts.append(tr)
+        keep.append(chunks)
         p = lambda a: a.ctypes.data if a.size else None
         descs[i] = VerifyProof(p(lr), lr.shape[0], p(delta), p(z1), p(z2), p(sg), p(elm), elm.shape[0], p(ps), p(es), p(cxy), chunks,
-                               len(comms), p(cip), ctypes.pointer(tr))
-    rng = np.concatenate([np.ascontiguousarray(rand_base, dtype=np.uint64).reshape(4), np.ascontiguousarray(sg_rand_base, dtype=np.uint64).reshape(4)])
+                               len(comms), p(cip), ctypes.pointer(tr.struct))
+    rng = np.concatenate([_fe(rand_base), _fe(sg_rand_base)])
     ok = ctypes.c_int(0)
     out = np.zeros(12, dtype=np.uint64)
     rc = lib().zk_srs_verify(srs._h, descs, len(batch), _ptr(rng), ctypes.byref(ok), _ptr(out))
-    if errors:
-        raise errors[0]
+    for tr in transcripts:
+        tr.reraise()
     check(rc)
     if not return_sum:
         return bool(ok.value)
-    from ._lib import jacobian_to_affine
     return bool(ok.value), jacobian_to_affine(srs.curve, out)
 
 
-class IpaRounds:
+class IpaRounds(Handle):
     """The folding loop of SRS::open (poly-commitment/src/ipa.rs:929-1007) with a and b resident on the device and the bases
     taken from the resident SRS table (`bases` = ctx.upload_bases(curve, srs.g)); see csrc/ipa.cu.
 
@@ -380,8 +348,7 @@ class IpaRounds:
         return l, r, ipl, ipr
 
     def fold(self, u_mont, u_inv_mont):
-        u = np.ascontiguousarray(u_mont, dtype=np.uint64).reshape(4)
-        ui = np.ascontiguousarray(u_inv_mont, dtype=np.uint64).reshape(4)
+        u, ui = _fe(u_mont), _fe(u_inv_mont)
         check(lib().zk_ipa_round_fold(self._h, u.ctypes.data_as(_u64p), ui.ctypes.data_as(_u64p)))
 
     def state(self):
@@ -396,17 +363,8 @@ class IpaRounds:
         check(lib().zk_ipa_read(self._h, None, None, 0, out.ctypes.data_as(_u64p)))
         return out
 
-    def close(self):
-        if getattr(self, "_h", None):
-            lib().zk_ipa_free(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            if self.ctx._h:
-                self.close()
-        except Exception:
-            pass
+    def _release(self, h):
+        lib().zk_ipa_free(h)
 
 
 class ExprProgram:
@@ -421,7 +379,7 @@ class ExprProgram:
         self.n_cached = 0
 
     def literal(self, x_mont):
-        self.constants.append(np.ascontiguousarray(x_mont, dtype=np.uint64).reshape(4))
+        self.constants.append(_fe(x_mont))
         self.tokens.append((self.CONST, len(self.constants) - 1)); return self
 
     def cell(self, col: int, next_row: bool = False):
@@ -500,7 +458,6 @@ class LookupSpec:
 
     def info(self, row_pattern, joint_combiner, table_id_combiner, dummy) -> "LookupInfo":
         """The zk_lookup_info of these patterns for rows row_pattern (uint8 [lookup_rows]: 0 none, p + 1 pattern p); scalars Montgomery"""
-        from ._lib import LookupInfo, LookupJoint, LookupTerm
         terms = (LookupTerm * max(1, len(self.terms)))()
         for k, (c, col, nxt) in enumerate(self.terms):
             terms[k].coeff[:] = list(c)
@@ -526,7 +483,7 @@ class LookupSpec:
         return s
 
 
-class LagrangeBasisEvaluations:
+class LagrangeBasisEvaluations(Handle):
     """kimchi::lagrange_basis_evaluations::LagrangeBasisEvaluations (lagrange_basis_evaluations.rs:24-258) resident on the device: the
     chunks x n basis values at x live in a device buffer this object owns (close() frees it).  Columns are (device pointer, len) pairs
     of Montgomery evaluations whose length is a multiple of domain_size()."""
@@ -534,7 +491,8 @@ class LagrangeBasisEvaluations:
     def __init__(self, ctx: Context, field: int, max_poly_size: int, log_n: int, x):
         self.ctx, self.field, self.log_n = ctx, field, log_n
         self.chunks = Context.lagrange_evals_chunks(1 << log_n, max_poly_size)
-        self.ptr = ctx.dev_alloc(max(1, self.chunks) << (log_n + 5))
+        self._h = ctx.buffers()
+        self.ptr = self._h.alloc(max(1, self.chunks) << (log_n + 5))
         try:
             ctx.lagrange_basis_evals_dev(field, log_n, max_poly_size, x, self.ptr)
         except Exception:
@@ -572,17 +530,8 @@ class LagrangeBasisEvaluations:
         """the basis values [chunks, n, 4] (downloaded)"""
         return self.ctx.dev_download(self.ptr, (self.chunks, self.domain_size(), 4))
 
-    def close(self):
-        if getattr(self, "ptr", None):
-            self.ctx.dev_free(self.ptr)
-            self.ptr = None
-
-    def __del__(self):
-        try:
-            if self.ctx._h:
-                self.close()
-        except Exception:
-            pass
+    def _release(self, bufs):
+        bufs.close()
 
 
 class Radix2EvaluationDomain:

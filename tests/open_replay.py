@@ -215,12 +215,9 @@ def opening_proof_bytes_product_level(orc, zk, ctx, vesta_srs) -> bytes:
         sponge.absorb_g([P.xy(delta)])
         return mont([scalar_challenge_to_field(sponge.challenge(), endo_r, FP)])[0]
 
-    srs = zk.SRS(ctx, zk.VESTA, g, h)
-    try:
+    with zk.SRS(ctx, zk.VESTA, g, h) as srs:
         plnms = [(mont(c), 0, mont(bl)) for c, bl in polys]
         proof = zk.srs_open(srs, plnms, mont(elm), mont([polyscale])[0], mont([evalscale])[0], mont(draws), u_base, round_challenge, final_challenge)
-    finally:
-        srs.close()
     pt = lambda p: b"\xc4\x21" + P.compress(p)
     fe = lambda x: b"\xc4\x20" + fe_int(x).to_bytes(32, "little")
     lr = proof.lr

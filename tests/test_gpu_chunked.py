@@ -12,6 +12,7 @@ result is compared bit for bit with the CPU oracle or the Python restatements (t
 verify_replay.py); where a restatement would hold a whole 2^20 x 16 basis in Python integers, the test uses the exact identity
 sum_i p[s i] l_{x,k}[i] = chunk k of interpolate(p[::s]) at x.  Each test runs on a context of its own and stays below about
 3 GiB of device memory and 6 GiB of host memory."""
+import contextlib
 import random
 
 import numpy as np
@@ -47,19 +48,6 @@ def srs(ctx, vesta_srs):
 
 def rnd(orc, fid, k, seed):
     return orc.to_mont(fid, orc.random_scalars(fid, k, seed=seed))
-
-
-def put(ctx, bufs, a):
-    a = np.ascontiguousarray(a, dtype=np.uint64)
-    p = ctx.dev_alloc(max(a.nbytes, 32))
-    bufs.append(p)
-    ctx.dev_upload(p, a)
-    return p
-
-
-def free_all(ctx, bufs):
-    for p in bufs:
-        ctx.dev_free(p)
 
 
 def m1(orc, fid, x):
@@ -182,18 +170,13 @@ def test_lagrange_evaluate_chunked_at_zeta_and_zeta_omega(ctx, orc, log_n):
     bits = np.random.default_rng(log_n).integers(0, 2, size=(4 * n, 1)) == 1
     sel = np.where(bits, rnd(orc, fid, 4 * n, 320 + log_n), np.uint64(0)).astype(np.uint64)   # nonzero values count as one
     ind = np.where(bits[::4], orc.fe(fid, 1), np.uint64(0)).astype(np.uint64)
-    bufs, lbs = [], []
-    try:
-        d = {s: put(ctx, bufs, c) for s, c in cols.items()}
-        d_sel = put(ctx, bufs, sel)
-        lbs = [zk.LagrangeBasisEvaluations(ctx, fid, M, log_n, m1(orc, fid, x)) for x in pts]
+    with ctx.buffers() as bufs, contextlib.ExitStack() as stack:
+        d = {s: bufs.put(c) for s, c in cols.items()}
+        d_sel = bufs.put(sel)
+        lbs = [stack.enter_context(zk.LagrangeBasisEvaluations(ctx, fid, M, log_n, m1(orc, fid, x))) for x in pts]
         assert lbs[0].chunks == nc
         got = zk.LagrangeBasisEvaluations.evaluate_all(lbs, [(d[s], s * n, False) for s in (1, 4, 8)] + [(d_sel, 4 * n, True)])
         basis17 = [lb.evals() for lb in lbs] if log_n == 17 else None
-    finally:
-        for lb in lbs:
-            lb.close()
-        free_all(ctx, bufs)
     assert got.shape == (4, 2, nc, 4)
     host = [cols[s][::s] for s in (1, 4, 8)] + [ind]
     if log_n == 17:
@@ -219,16 +202,11 @@ def test_lagrange_evaluate_partial_second_pair_group(ctx, orc, fid):
     pts = [rng.randrange(P) for _ in range(3)]
     c1, c8 = [rng.randrange(P) for _ in range(n)], [rng.randrange(P) for _ in range(8 * n)]
     bits = [rng.randrange(2) * rng.randrange(1, P) for _ in range(n)]
-    bufs, lbs = [], []
-    try:
-        cols = [(put(ctx, bufs, ev.mont(orc, fid, c1)), n, False), (put(ctx, bufs, ev.mont(orc, fid, c8)), 8 * n, False),
-                (put(ctx, bufs, ev.mont(orc, fid, bits)), n, True)]
-        lbs = [zk.LagrangeBasisEvaluations(ctx, fid, m, log_n, m1(orc, fid, x)) for x in pts]
+    with ctx.buffers() as bufs, contextlib.ExitStack() as stack:
+        cols = [(bufs.put(ev.mont(orc, fid, c1)), n, False), (bufs.put(ev.mont(orc, fid, c8)), 8 * n, False),
+                (bufs.put(ev.mont(orc, fid, bits)), n, True)]
+        lbs = [stack.enter_context(zk.LagrangeBasisEvaluations(ctx, fid, m, log_n, m1(orc, fid, x))) for x in pts]
         got = zk.LagrangeBasisEvaluations.evaluate_all(lbs, cols)
-    finally:
-        for lb in lbs:
-            lb.close()
-        free_all(ctx, bufs)
     assert got.shape == (3, 3, 4, 4)
     for t, x in enumerate(pts):
         basis = ev.lagrange_basis(orc, fid, m, log_n, x)
@@ -249,13 +227,10 @@ def test_evaluate_chunks_several_point_groups(ctx, orc, nc):
     lens = [nc * M, (nc - 1) * M + 777, 1000]
     polys = [canonical_ints(orc.random_scalars(fid, k, seed=51 + k)) for k in lens]
     pts = [0, 1] + [rng.randrange(P) for _ in range(7)]
-    bufs = []
-    try:
-        desc = [(put(ctx, bufs, ev.mont(orc, fid, p)), len(p)) for p in polys]
+    with ctx.buffers() as bufs:
+        desc = [(bufs.put(ev.mont(orc, fid, p)), len(p)) for p in polys]
         got9 = ctx.poly_evaluate_chunks_dev(fid, desc, nc, M, ev.mont(orc, fid, pts))
         got5 = ctx.poly_evaluate_chunks_dev(fid, desc, nc, M, ev.mont(orc, fid, pts[:5]))
-    finally:
-        free_all(ctx, bufs)
     assert got9.shape == (3, 9, nc, 4) and got5.shape == (3, 5, nc, 4)
     assert np.array_equal(got5, got9[:, :5])
     for j, p in enumerate(polys):
@@ -275,15 +250,10 @@ def test_lagrange_evaluate_more_than_65535_outputs(ctx, orc):
     a = [rng.randrange(P) for _ in range(n)]
     b = [rng.randrange(2) * rng.randrange(1, P) for _ in range(2 * n)]
     n_cols = 4097
-    bufs, lbs = [], []
-    try:
-        d_a, d_b = put(ctx, bufs, ev.mont(orc, fid, a)), put(ctx, bufs, ev.mont(orc, fid, b))
-        lbs = [zk.LagrangeBasisEvaluations(ctx, fid, m, log_n, m1(orc, fid, x)) for x in pts]
+    with ctx.buffers() as bufs, contextlib.ExitStack() as stack:
+        d_a, d_b = bufs.put(ev.mont(orc, fid, a)), bufs.put(ev.mont(orc, fid, b))
+        lbs = [stack.enter_context(zk.LagrangeBasisEvaluations(ctx, fid, m, log_n, m1(orc, fid, x))) for x in pts]
         got = zk.LagrangeBasisEvaluations.evaluate_all(lbs, [(d_a, n, False) if j % 2 == 0 else (d_b, 2 * n, True) for j in range(n_cols)])
-    finally:
-        for lb in lbs:
-            lb.close()
-        free_all(ctx, bufs)
     assert got.shape == (n_cols, 2, 8, 4) and got.shape[0] * 16 > 65535
     bases = [ev.lagrange_basis(orc, fid, m, log_n, x) for x in pts]
     want_a = np.stack([ev.mont(orc, fid, ev.evaluate(bs, a, P)) for bs in bases])
@@ -302,13 +272,10 @@ def test_evaluate_chunks_more_than_65535_outputs(ctx, orc):
     a = [rng.randrange(P) for _ in range(nc * cs)]
     b = [rng.randrange(P) for _ in range(1000)]
     n_polys = 821
-    bufs = []
-    try:
-        d_a, d_b = put(ctx, bufs, ev.mont(orc, fid, a)), put(ctx, bufs, ev.mont(orc, fid, b))
+    with ctx.buffers() as bufs:
+        d_a, d_b = bufs.put(ev.mont(orc, fid, a)), bufs.put(ev.mont(orc, fid, b))
         got = ctx.poly_evaluate_chunks_dev(fid, [(d_a, len(a)) if j % 2 == 0 else (d_b, len(b)) for j in range(n_polys)], nc, cs,
                                            ev.mont(orc, fid, pts))
-    finally:
-        free_all(ctx, bufs)
     assert got.shape == (n_polys, 5, nc, 4) and n_polys * 5 * nc > 65535
     want_a = np.stack([ev.mont(orc, fid, ev.evaluate_chunks(a, nc, cs, x, P)) for x in pts])
     want_b = np.stack([ev.mont(orc, fid, ev.evaluate_chunks(b, nc, cs, x, P)) for x in pts])
@@ -331,19 +298,16 @@ def test_ft_chunked(ctx, orc, log_n):
     s6_8 = rnd(orc, fid, 8 * n, 71 + log_n)
     terms = [(ev.ints(orc, fid, s6_8[::8]), perm)]                 # the entries the device reads: combine_terms at stride 1
     t_full = orc.random_scalars(fid, 7 * nc * M, seed=72 + log_n)
-    bufs = []
-    try:
-        d_s8 = put(ctx, bufs, s6_8)
+    with ctx.buffers() as bufs:
+        d_s8 = bufs.put(s6_8)
         del s6_8
-        d_t = put(ctx, bufs, orc.to_mont(fid, t_full))
-        d_ft = put(ctx, bufs, stale(M))
+        d_t = bufs.put(orc.to_mont(fid, t_full))
+        d_ft = bufs.put(stale(M))
         for t_len in (7 * nc * M, 7 * nc * M - M // 2 - 3):
             ctx.dev_upload(d_ft, stale(M))
             ft_len, e1 = ctx.prover_ft_dev(fid, log_n, M, [(d_s8, 8 * n, m1(orc, fid, perm))], d_t, t_len, m1(orc, fid, zeta), d_ft)
             coeffs = ctx.dev_download(d_ft, (M, 4))
             check_against_replay(orc, fid, log_n, M, terms, canonical_ints(t_full[:t_len]), zeta, (coeffs, ft_len, e1))
-    finally:
-        free_all(ctx, bufs)
 
 
 # ---------------------------------------------------------------------------------------------------------------- opening and verification
@@ -444,10 +408,9 @@ def test_open_and_verify_chunked(ctx, orc, vesta_srs, srs):
              srs.commit_custom(q3, 16, ev.mont(orc, fid, bl[2])).chunks]
     assert [c.shape[0] for c in comms] == [2, 16, 16]
     del q3
-    bufs = []
-    entries = []
-    try:
-        d1, d2, d3 = put(ctx, bufs, orc.to_mont(fid, p1)), put(ctx, bufs, orc.to_mont(fid, p2)), put(ctx, bufs, ev8)
+    with ctx.buffers() as bufs:
+        entries = []
+        d1, d2, d3 = bufs.put(orc.to_mont(fid, p1)), bufs.put(orc.to_mont(fid, p2)), bufs.put(ev8)
         del ev8
         plnms = [((d1, 1 << 17), 0, ev.mont(orc, fid, bl[0])), ((d2, big), 0, ev.mont(orc, fid, bl[1])),
                  ((d3, 8 * big), big, ev.mont(orc, fid, bl[2]))]
@@ -456,8 +419,6 @@ def test_open_and_verify_chunked(ctx, orc, vesta_srs, srs):
             e = open_and_check(orc, G, srs, plnms, host, sc[:2], sc[2], sc[3], sc[4:], 800 + k)
             e.comms = comms
             entries.append(e)
-    finally:
-        free_all(ctx, bufs)
     rb, sgb = rng.randrange(P), rng.randrange(P)
     batch = lambda es: [to_device(zk, orc, fid, e) for e in es]
     ok, pt = zk.srs_verify(srs, batch(entries), m1(orc, fid, rb), m1(orc, fid, sgb), return_sum=True)

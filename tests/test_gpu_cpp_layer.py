@@ -82,8 +82,7 @@ def test_cpp_host_layer_matches_the_oracle(orc, pallas_srs, tmp_path):
     # OpenProof::open through the C++ layer == the same call through the ctypes layer (itself pinned to the reference's 700-byte
     # opening proof in tests/test_gpu_srs.py), same stand-in sponge: U = g[7], every challenge = u
     import proof_systems_b200 as zk
-    ctx = zk.Context(0)
-    try:
+    with zk.Context(0) as ctx:
         srs = zk.SRS(ctx, G.cid, g, h)
         um, uim = mont([u])[0], mont([pow(u, -1, m)])[0]
         pr = zk.srs_open(srs, [(mont(coeffs_i[:n]), 0, mont(blind_i[:1]))], np.stack([um, uim]), um, uim, mont(evals_i[:2 * k + 2]),
@@ -92,5 +91,3 @@ def test_cpp_host_layer_matches_the_oracle(orc, pallas_srs, tmp_path):
         assert np.array_equal(open_pts[2], pr.delta) and np.array_equal(open_pts[3], pr.sg)
         assert np.array_equal(open_z[0], pr.z1) and np.array_equal(open_z[1], pr.z2)
         srs.close()
-    finally:
-        ctx.close()

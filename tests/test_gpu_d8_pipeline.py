@@ -25,16 +25,11 @@ def test_permutation_quotient_kernel_vs_oracle(ctx, orc, fid, log_m):
     z, zkpm = rnd(m, 3), rnd(m, 4)
     beta, gamma, alpha0, shifts = rnd(1, 5)[0], rnd(1, 6)[0], rnd(1, 7)[0], rnd(7, 8)
     want = orc.perm_quot(fid, w, z, sigma, zkpm, beta, gamma, alpha0, shifts)
-    bufs = {k: ctx.dev_alloc(v.nbytes) for k, v in (("w", w), ("sigma", sigma), ("z", z), ("zkpm", zkpm), ("out", z))}
-    try:
-        for k, v in (("w", w), ("sigma", sigma), ("z", z), ("zkpm", zkpm)):
-            ctx.dev_upload(bufs[k], v)
+    with ctx.buffers() as bufs:
+        d_w, d_sigma, d_z, d_zkpm, d_out = bufs.put(w), bufs.put(sigma), bufs.put(z), bufs.put(zkpm), bufs.alloc(z.nbytes)
         cols = lambda base: [base + k * m * 32 for k in range(7)]
-        ctx.perm_quotient_dev(fid, log_m, cols(bufs["w"]), bufs["z"], cols(bufs["sigma"]), bufs["zkpm"], beta, gamma, alpha0, shifts, bufs["out"])
-        assert np.array_equal(ctx.dev_download(bufs["out"], (m, 4)), want)
-    finally:
-        for p in bufs.values():
-            ctx.dev_free(p)
+        ctx.perm_quotient_dev(fid, log_m, cols(d_w), d_z, cols(d_sigma), d_zkpm, beta, gamma, alpha0, shifts, d_out)
+        assert np.array_equal(ctx.dev_download(d_out, (m, 4)), want)
 
 
 def test_device_resident_d8_pipeline(ctx, orc):
@@ -58,9 +53,9 @@ def test_device_resident_d8_pipeline(ctx, orc):
     perm = orc.perm_quot(fid, ev8[:7], ev8[7], sigma8, zkpm, beta, gamma, alpha0, shifts)
     want = orc.ntt(fid, perm, inverse=True)
     # ---- device
-    d_cols, d_ev8 = ctx.dev_alloc(cols.nbytes), ctx.dev_alloc(8 * m * 32)
-    d_sigma, d_zkpm, d_out = ctx.dev_alloc(sigma8.nbytes), ctx.dev_alloc(zkpm.nbytes), ctx.dev_alloc(m * 32)
-    try:
+    with ctx.buffers() as bufs:
+        d_cols, d_ev8 = bufs.alloc(cols.nbytes), bufs.alloc(8 * m * 32)
+        d_sigma, d_zkpm, d_out = bufs.alloc(sigma8.nbytes), bufs.alloc(zkpm.nbytes), bufs.alloc(m * 32)
         launches0 = ctx.launch_count
         ctx.dev_upload(d_cols, cols)
         ctx.dev_upload(d_sigma, sigma8)
@@ -73,6 +68,3 @@ def test_device_resident_d8_pipeline(ctx, orc):
         got = ctx.dev_download(d_out, (m, 4))
         assert np.array_equal(got, want)
         assert ctx.launch_count - launches0 >= 6
-    finally:
-        for p in (d_cols, d_ev8, d_sigma, d_zkpm, d_out):
-            ctx.dev_free(p)

@@ -1,6 +1,7 @@
 """The prover's evaluations at zeta and zeta*omega on the device (kimchi/src/prover.rs:1009-1058): zk_lagrange_evals_dev,
 zk_lagrange_evaluate_dev and zk_poly_evaluate_chunks_dev, every result compared bit for bit with the Python restatement of
 LagrangeBasisEvaluations / evaluate_chunks (tests/evals_replay.py)."""
+import contextlib
 import random
 import threading
 
@@ -20,25 +21,9 @@ def ctx():
     c.close()
 
 
-def put(ctx, bufs, a):
-    a = np.ascontiguousarray(a, dtype=np.uint64)
-    p = ctx.dev_alloc(max(a.nbytes, 32))
-    bufs.append(p)
-    ctx.dev_upload(p, a)
-    return p
-
-
-def free_all(ctx, bufs):
-    for p in bufs:
-        ctx.dev_free(p)
-
-
 def device_basis(ctx, orc, fid, m, log_n, x):
-    lb = zk.LagrangeBasisEvaluations.new(ctx, fid, m, log_n, ev.mont(orc, fid, [x])[0])
-    try:
+    with zk.LagrangeBasisEvaluations.new(ctx, fid, m, log_n, ev.mont(orc, fid, [x])[0]) as lb:
         return lb.chunks, lb.evals()
-    finally:
-        lb.close()
 
 
 def expected_basis(orc, fid, m, log_n, x):
@@ -95,9 +80,9 @@ def test_evaluate_two_points_in_one_call(ctx, orc, fid, chunks):
     zeta = rng.randrange(P)
     pts = [zeta, zeta * ev.omega(orc, fid, log_n) % P]
     cols = {s: [rng.randrange(P) for _ in range(s * n)] for s in (1, 4, 8)}
-    bufs, lbs = [], [zk.LagrangeBasisEvaluations(ctx, fid, n // chunks, log_n, ev.mont(orc, fid, [x])[0]) for x in pts]
-    try:
-        d = {s: put(ctx, bufs, ev.mont(orc, fid, c)) for s, c in cols.items()}
+    with ctx.buffers() as bufs, contextlib.ExitStack() as stack:
+        lbs = [stack.enter_context(zk.LagrangeBasisEvaluations(ctx, fid, n // chunks, log_n, ev.mont(orc, fid, [x])[0])) for x in pts]
+        d = {s: bufs.put(ev.mont(orc, fid, c)) for s, c in cols.items()}
         got = zk.LagrangeBasisEvaluations.evaluate_all(lbs, [(d[s], s * n, False) for s in (1, 4, 8)])
         assert got.shape == (3, 2, chunks, 4)
         for j, s in enumerate((1, 4, 8)):
@@ -105,10 +90,6 @@ def test_evaluate_two_points_in_one_call(ctx, orc, fid, chunks):
                 want = ev.evaluate(ev.lagrange_basis(orc, fid, n // chunks, log_n, x), cols[s], P)
                 assert np.array_equal(got[j, t], ev.mont(orc, fid, want)), (s, t)
         assert np.array_equal(lbs[1].evaluate((d[4], 4 * n)), got[1, 1])
-    finally:
-        for lb in lbs:
-            lb.close()
-        free_all(ctx, bufs)
 
 
 @pytest.mark.parametrize("fid", [0, 1])
@@ -122,18 +103,14 @@ def test_evaluate_boolean(ctx, orc, fid, chunks):
     bits = [rng.randrange(2) for _ in range(4 * n)]
     other = [rng.choice([0, 1, 2, P - 1, rng.randrange(P)]) for _ in range(n)]
     basis = ev.lagrange_basis(orc, fid, n // chunks, log_n, x)
-    bufs, lb = [], zk.LagrangeBasisEvaluations(ctx, fid, n // chunks, log_n, ev.mont(orc, fid, [x])[0])
-    try:
-        d_bits, d_other = put(ctx, bufs, ev.mont(orc, fid, bits)), put(ctx, bufs, ev.mont(orc, fid, other))
+    with ctx.buffers() as bufs, zk.LagrangeBasisEvaluations(ctx, fid, n // chunks, log_n, ev.mont(orc, fid, [x])[0]) as lb:
+        d_bits, d_other = bufs.put(ev.mont(orc, fid, bits)), bufs.put(ev.mont(orc, fid, other))
         assert np.array_equal(lb.evaluate_boolean((d_bits, 4 * n)), ev.mont(orc, fid, ev.evaluate_boolean(basis, bits, P)))
         got = lb.evaluate_boolean((d_other, n))
         assert np.array_equal(got, ev.mont(orc, fid, ev.evaluate_boolean(basis, other, P)))
         assert not np.array_equal(got, lb.evaluate((d_other, n)))
         both = ctx.lagrange_evaluate_dev(fid, [lb.ptr], log_n, lb.chunks, [(d_other, n, True), (d_other, n, False)])
         assert np.array_equal(both[0, 0], got) and np.array_equal(both[1, 0], ev.mont(orc, fid, ev.evaluate(basis, other, P)))
-    finally:
-        lb.close()
-        free_all(ctx, bufs)
 
 
 # ---------------------------------------------------------------------------------------------------------------- evaluate_chunks
@@ -145,9 +122,8 @@ def test_evaluate_chunks(ctx, orc, fid, num_chunks, chunk_size):
     lens = [0, 1, chunk_size - 3, num_chunks * chunk_size, max(0, (num_chunks - 1) * chunk_size - 5)]
     polys = [[rng.randrange(P) for _ in range(k)] for k in lens]
     pts = [0, 1, rng.randrange(P)]
-    bufs = []
-    try:
-        desc = [(put(ctx, bufs, ev.mont(orc, fid, p)) if p else 0, len(p)) for p in polys]
+    with ctx.buffers() as bufs:
+        desc = [(bufs.put(ev.mont(orc, fid, p)) if p else 0, len(p)) for p in polys]
         got = ctx.poly_evaluate_chunks_dev(fid, desc, num_chunks, chunk_size, ev.mont(orc, fid, pts))
         assert got.shape == (len(polys), len(pts), num_chunks, 4)
         for j, p in enumerate(polys):
@@ -156,8 +132,6 @@ def test_evaluate_chunks(ctx, orc, fid, num_chunks, chunk_size):
         with pytest.raises(zk.ZkError) as e:
             ctx.poly_evaluate_chunks_dev(fid, desc[3:4], num_chunks - 1, chunk_size, ev.mont(orc, fid, pts))
         assert e.value.code == -4                                                   # ZK_ERR_LENGTH
-    finally:
-        free_all(ctx, bufs)
 
 
 # ---------------------------------------------------------------------------------------------------------------- the prover's step
@@ -184,25 +158,19 @@ def test_prover_step_at_zeta_and_zeta_omega(ctx, orc):
     want_l = [[ev.evaluate(b, h, P) if k < 22 else ev.evaluate_boolean(b, h, P) for b in bases] for k, h in enumerate(host)]
     want_c = [[ev.evaluate_chunks(c, 1, n, x, P) for x in pts] for c in coeffs]
     # ---------------------------------------------------------------- device
-    bufs = []
-    lbs = []
-    try:
-        d_cols = put(ctx, bufs, cols)
-        d_s8, d_c8 = put(ctx, bufs, s8), put(ctx, bufs, c8)
-        d_sel = [put(ctx, bufs, s) for s in sel]
-        d_w8 = ctx.dev_alloc(15 * 8 * n * 32); bufs.append(d_w8)
+    with ctx.buffers() as bufs, contextlib.ExitStack() as stack:
+        d_cols = bufs.put(cols)
+        d_s8, d_c8 = bufs.put(s8), bufs.put(c8)
+        d_sel = [bufs.put(s) for s in sel]
+        d_w8 = bufs.alloc(15 * 8 * n * 32)
         ctx.ntt_dev(fid, d_cols, log_n, batch=17, inverse=True)                      # prover.rs:370-381: the columns' coefficients
         ctx.ntt_dev_oop(fid, d_cols, n, n, d_w8, log_n + 3, batch=15)                 # constraints.rs:488-507: witness over d8
-        lbs = [zk.LagrangeBasisEvaluations(ctx, fid, n, log_n, ev.mont(orc, fid, [x])[0]) for x in pts]
+        lbs = [stack.enter_context(zk.LagrangeBasisEvaluations(ctx, fid, n, log_n, ev.mont(orc, fid, [x])[0])) for x in pts]
         columns = [(d_s8 + k * 8 * n * 32, 8 * n, False) for k in range(7)] + [(d_c8 + k * 8 * n * 32, 8 * n, False) for k in range(15)]
         columns += [(d, s.shape[0], True) for d, s in zip(d_sel, sel)]
         columns += [(d_w8 + k * 8 * n * 32, 8 * n, False) for k in range(15)]
         got_l = zk.LagrangeBasisEvaluations.evaluate_all(lbs, columns)
         got_c = ctx.poly_evaluate_chunks_dev(fid, [(d_cols + j * n * 32, n) for j in range(17)], 1, n, ev.mont(orc, fid, pts))
-    finally:
-        for lb in lbs:
-            lb.close()
-        free_all(ctx, bufs)
     for k in range(28):
         for t in range(2):
             assert np.array_equal(got_l[k, t], ev.mont(orc, fid, want_l[k][t])), (k, t)
@@ -219,9 +187,8 @@ def test_errors(ctx, orc):
     P = orc.MODULUS[fid]
     x = ev.mont(orc, fid, [5])[0]
     bad_x = np.array([P & (2**64 - 1), (P >> 64) & (2**64 - 1), (P >> 128) & (2**64 - 1), P >> 192], dtype=np.uint64)
-    bufs = []
-    try:
-        d = ctx.dev_alloc(64 * 32); bufs.append(d)
+    with ctx.buffers() as bufs:
+        d = bufs.alloc(64 * 32)
         inv = lambda f: pytest.raises(zk.ZkError, match="error -1")
         with inv(0): ctx.lagrange_basis_evals_dev(7, 4, 16, x, d)                     # unknown field
         with inv(0): ctx.lagrange_basis_evals_dev(fid, 31, 16, x, d)                  # log_n > 30
@@ -249,8 +216,6 @@ def test_errors(ctx, orc):
             ctx.poly_evaluate_chunks_dev(fid, [(d, 17)], 1, 16, [x])
         assert e.value.code == -4 and "more than 1 chunks of 16" in str(e.value)
         assert ctx.poly_evaluate_chunks_dev(fid, [(d, 16)], 1, 16, [x]).shape == (1, 1, 1, 4)
-    finally:
-        free_all(ctx, bufs)
 
 
 def test_two_threads_share_a_context(ctx, orc):
@@ -261,31 +226,25 @@ def test_two_threads_share_a_context(ctx, orc):
     coeffs = [rng.randrange(P) for _ in range(n)]
     xs = [rng.randrange(P) for _ in range(2)]
     want = [(ev.evaluate(ev.lagrange_basis(orc, fid, n // 2, log_n, x), col, P), ev.evaluate_chunks(coeffs, 2, n // 2, x, P)) for x in xs]
-    bufs = []
-    d_col, d_coeffs = put(ctx, bufs, ev.mont(orc, fid, col)), put(ctx, bufs, ev.mont(orc, fid, coeffs))
     errors = []
 
     def work(t):
         try:
             xm = ev.mont(orc, fid, [xs[t]])
             for _ in range(6):
-                lb = zk.LagrangeBasisEvaluations(ctx, fid, n // 2, log_n, xm[0])
-                try:
+                with zk.LagrangeBasisEvaluations(ctx, fid, n // 2, log_n, xm[0]) as lb:
                     got = lb.evaluate((d_col, 4 * n))
-                finally:
-                    lb.close()
                 assert np.array_equal(got, ev.mont(orc, fid, want[t][0]))
                 got = ctx.poly_evaluate_chunks_dev(fid, [(d_coeffs, n)], 2, n // 2, xm)[0, 0]
                 assert np.array_equal(got, ev.mont(orc, fid, want[t][1]))
         except Exception as e:                    # reported by the main thread
             errors.append(e)
 
-    try:
+    with ctx.buffers() as bufs:
+        d_col, d_coeffs = bufs.put(ev.mont(orc, fid, col)), bufs.put(ev.mont(orc, fid, coeffs))
         th = [threading.Thread(target=work, args=(t,)) for t in range(2)]
         for t in th:
             t.start()
         for t in th:
             t.join()
-    finally:
-        free_all(ctx, bufs)
     assert not errors, errors

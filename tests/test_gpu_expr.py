@@ -21,19 +21,6 @@ def ctx():
     c.close()
 
 
-class Resident:
-    """columns uploaded once; frees on exit"""
-    def __init__(self, ctx):
-        self.ctx, self.ptrs = ctx, []
-    def put(self, a):
-        p = self.ctx.dev_alloc(a.nbytes); self.ptrs.append(p); self.ctx.dev_upload(p, a); return p
-    def alloc(self, nbytes):
-        p = self.ctx.dev_alloc(nbytes); self.ptrs.append(p); return p
-    def __enter__(self): return self
-    def __exit__(self, *a):
-        for p in self.ptrs: self.ctx.dev_free(p)
-
-
 def _columns(orc, fid, log_n, seed):
     n, m = 1 << log_n, 8 << log_n
     rnd = lambda k, s: orc.to_mont(fid, orc.random_scalars(fid, k, seed=s))
@@ -46,7 +33,7 @@ def test_generic_gate_over_d4(ctx, orc, fid, log_n):
     sel4, alphas = rnd(4 * n, 900), rnd(2, 901)
     rec = gp.generic_gate(gp.Recorder(), alphas)
     want = orc.expr_eval(fid, rec.ops, rec.args, rec.literals, [(a, 8) for a in w + co] + [(sel4, 4)], 4 * n)
-    with Resident(ctx) as r:
+    with ctx.buffers() as r:
         cols = [(r.put(a), m, 8) for a in w + co] + [(r.put(sel4), 4 * n, 4)]
         d_out = r.alloc(4 * n * 32)
         prog = gp.generic_gate(zk.ExprProgram(), alphas)
@@ -62,7 +49,7 @@ def test_complete_add_gate_over_d4(ctx, orc, fid, log_n):
     one = orc.to_mont(fid, orc.ints_to_limbs([1]))[0]
     rec = gp.complete_add_gate(gp.Recorder(), alphas, one)
     want = orc.expr_eval(fid, rec.ops, rec.args, rec.literals, [(a, 8) for a in w + co] + [(sel4, 4)], 4 * n)
-    with Resident(ctx) as r:
+    with ctx.buffers() as r:
         cols = [(r.put(a), m, 8) for a in w + co] + [(r.put(sel4), 4 * n, 4)]
         d_out = r.alloc(4 * n * 32)
         gp.complete_add_gate(zk.ExprProgram(), alphas, one).evaluations(ctx, fid, cols, 4 * n, 4, d_out)
@@ -83,7 +70,7 @@ def test_endomul_scalar_gate_over_d8(ctx, orc, fid, log_n):
     sel8, alphas = rnd(m, 970), rnd(11, 971)
     rec = gp.endomul_scalar_gate(gp.Recorder(), alphas, _Lit(orc, fid))
     want = orc.expr_eval(fid, rec.ops, rec.args, rec.literals, [(a, 8) for a in w + co] + [(sel8, 8)], m)
-    with Resident(ctx) as r:
+    with ctx.buffers() as r:
         cols = [(r.put(a), m, 8) for a in w + co] + [(r.put(sel8), m, 8)]
         d_out = r.alloc(m * 32)
         gp.endomul_scalar_gate(zk.ExprProgram(), alphas, _Lit(orc, fid)).evaluations(ctx, fid, cols, m, 8, d_out)
@@ -99,7 +86,7 @@ def test_endomul_gate_over_d8(ctx, orc, fid, log_n):
     one = orc.to_mont(fid, orc.ints_to_limbs([1]))[0]
     rec = gp.endomul_gate(gp.Recorder(), alphas, one, endo)
     want = orc.expr_eval(fid, rec.ops, rec.args, rec.literals, [(a, 8) for a in w + co] + [(sel8, 8)], m)
-    with Resident(ctx) as r:
+    with ctx.buffers() as r:
         cols = [(r.put(a), m, 8) for a in w + co] + [(r.put(sel8), m, 8)]
         d_out = r.alloc(m * 32)
         gp.endomul_gate(zk.ExprProgram(), alphas, one, endo).evaluations(ctx, fid, cols, m, 8, d_out)
@@ -115,7 +102,7 @@ def test_poseidon_gate_over_d8_and_accumulation_into_t8(ctx, orc, fid, log_n):
     cols_h = [(a, 8) for a in w + co] + [(sel8, 8)]
     want = orc.expr_eval(fid, rec.ops, rec.args, rec.literals, cols_h, m)
     want_acc = orc.expr_eval(fid, rec.ops, rec.args, rec.literals, cols_h, m, acc=t8)
-    with Resident(ctx) as r:
+    with ctx.buffers() as r:
         cols = [(r.put(a), m, 8) for a in w + co] + [(r.put(sel8), m, 8)]
         d_out, d_t8 = r.alloc(m * 32), r.put(t8)
         prog = gp.poseidon_gate(zk.ExprProgram(), alphas, mds)
@@ -164,7 +151,7 @@ def test_random_programs_use_every_opcode_and_mixed_domains(ctx, orc, seed):
     rec = _random_program(rng, len(cols_h), 5, 120)
     assert set(rec.ops) == set(range(9))
     want = orc.expr_eval(fid, rec.ops, rec.args, lits, cols_h, out_mult * n)
-    with Resident(ctx) as r:
+    with ctx.buffers() as r:
         cols = [(r.put(a), a.shape[0], cm) for a, cm in cols_h]
         d_out = r.alloc(out_mult * n * 32)
         ctx.expr_eval_dev(fid, list(zip(rec.ops, rec.args)), lits, cols, out_mult * n, out_mult, d_out)
@@ -196,7 +183,7 @@ def test_permutation_quotient_as_a_program_equals_the_dedicated_kernel(ctx, orc)
     for k in range(7):
         p.cell(Wc + k).literal(gamma).add().literal(beta).cell(S + k).mul().add().mul()
     p.sub().literal(alpha0).mul().cell(ZK).mul()
-    with Resident(ctx) as r:
+    with ctx.buffers() as r:
         cols = [(r.put(w[k]), m, 8) for k in range(7)] + [(r.put(sigma[k]), m, 8) for k in range(7)] + [(r.put(z), m, 8), (r.put(zkpm), m, 8), (r.put(x_col), m, 8)]
         d_out, d_out2 = r.alloc(m * 32), r.alloc(m * 32)
         p.evaluations(ctx, fid, cols, m, 8, d_out)
@@ -208,7 +195,7 @@ def test_permutation_quotient_as_a_program_equals_the_dedicated_kernel(ctx, orc)
 
 def test_malformed_programs_are_refused_before_anything_runs(ctx, orc):
     one = orc.to_mont(zk.FP, orc.ints_to_limbs([1]))
-    with Resident(ctx) as r:
+    with ctx.buffers() as r:
         col = [(r.put(orc.to_mont(zk.FP, orc.random_scalars(zk.FP, 16, seed=3))), 16, 8)]
         d_out = r.alloc(16 * 32)
         E = zk.ExprProgram

@@ -3,6 +3,7 @@ with the Python restatement (tests/ft_replay.py) — the m coefficients (zero pa
 fields, unchunked, n < m and chunked shapes, edge lengths of t, special points and cancellations; the verifier's ft_comm against
 commit(ft) masked with blinding_ft; one proof's tail from the resident quotient to an opening proof that zk_srs_verify accepts;
 errors and two threads on one context."""
+import contextlib
 import ctypes
 import random
 import threading
@@ -27,20 +28,6 @@ def ctx():
     c.close()
 
 
-def put(ctx, bufs, a):
-    a = np.ascontiguousarray(a, dtype=np.uint64)
-    p = ctx.dev_alloc(max(a.nbytes, 32))
-    bufs.append(p)
-    if a.nbytes:
-        ctx.dev_upload(p, a)
-    return p
-
-
-def free_all(ctx, bufs):
-    for p in bufs:
-        ctx.dev_free(p)
-
-
 def m1(orc, fid, x):
     return ev.mont(orc, fid, [x])[0]
 
@@ -52,9 +39,9 @@ def stale(m):
 
 def device_ft(ctx, orc, fid, log_n, m, terms, t, zeta, bufs):
     """upload terms / t, run the call over a stale ft buffer -> (ft [m, 4] Montgomery, ft_len, ft_eval1 [4], d_ft, d_t)"""
-    d_terms = [(put(ctx, bufs, ev.mont(orc, fid, e)), len(e), m1(orc, fid, c)) for e, c in terms]
-    d_t = put(ctx, bufs, ev.mont(orc, fid, t)) if t else 0
-    d_ft = put(ctx, bufs, stale(m))
+    d_terms = [(bufs.put(ev.mont(orc, fid, e)), len(e), m1(orc, fid, c)) for e, c in terms]
+    d_t = bufs.put(ev.mont(orc, fid, t)) if t else 0
+    d_ft = bufs.put(stale(m))
     ft_len, e1 = ctx.prover_ft_dev(fid, log_n, m, d_terms, d_t, len(t), m1(orc, fid, zeta), d_ft)
     return ctx.dev_download(d_ft, (m, 4)), ft_len, e1, d_ft, d_t
 
@@ -94,8 +81,7 @@ def test_ft_matches_the_reference(ctx, orc, fid, log_n, m, kind):
     zeta = rng.randrange(P)
     for t_len in (0, 1, m - 1, 7 * nc * m, 7 * nc * m - m // 2 - 3):
         t = [rng.randrange(P) for _ in range(t_len)]
-        bufs = []
-        try:
+        with ctx.buffers() as bufs:
             got = device_ft(ctx, orc, fid, log_n, m, terms, t, zeta, bufs)
             check_against_replay(orc, fid, log_n, m, terms, t, zeta, got)
             # ft_eval1 is evaluate_chunks of the resident ft at zeta omega
@@ -105,8 +91,6 @@ def test_ft_matches_the_reference(ctx, orc, fid, log_n, m, kind):
                 assert np.array_equal(again[0, 0, 0], got[2]), t_len
             else:
                 assert not got[2].any()
-        finally:
-            free_all(ctx, bufs)
 
 
 @pytest.mark.parametrize("fid", [0, 1])
@@ -120,8 +104,7 @@ def test_special_points(ctx, orc, fid, log_n, m):
     t = [rng.randrange(P) for _ in range(7 * nc * m - 5)]
     w3 = pow(ev.omega(orc, fid, log_n), 3, P)
     for zeta in (0, 1, w3):
-        bufs = []
-        try:
+        with ctx.buffers() as bufs:
             got = device_ft(ctx, orc, fid, log_n, m, terms, t, zeta, bufs)
             f, want = check_against_replay(orc, fid, log_n, m, terms, t, zeta, got)
             if zeta == 0:                             # ft = f_0 + t_0
@@ -129,8 +112,6 @@ def test_special_points(ctx, orc, fid, log_n, m):
                 assert want == fr.trim([(a + b) % P for a, b in zip(f0, t0)])
             else:
                 assert want == fr.linearize(fr.to_chunked_polynomial(f, nc, m), m, pow(zeta, m, P), P)
-        finally:
-            free_all(ctx, bufs)
 
 
 @pytest.mark.parametrize("fid", [0, 1])
@@ -149,15 +130,12 @@ def test_cancellation(ctx, orc, fid, log_n, m):
     t_part = list(t_cancel)
     t_part[5] = (t_part[5] + 3) % P
     for t, want_len in ((t_cancel, 0), (t_part, 6), (t_cancel[:len(t_cancel) - 4], len(lin_f))):
-        bufs = []
-        try:
+        with ctx.buffers() as bufs:
             got = device_ft(ctx, orc, fid, log_n, m, terms, t, zeta, bufs)
             check_against_replay(orc, fid, log_n, m, terms, t, zeta, got)
             assert got[1] == want_len and 0 <= want_len <= m
             if want_len == 0:
                 assert not got[0].any() and not got[2].any()
-        finally:
-            free_all(ctx, bufs)
 
 
 # ---------------------------------------------------------------------------------------------------------------- commitments
@@ -199,22 +177,18 @@ def test_commitment_equals_the_verifiers_ft_comm(ctx, orc, vesta_srs, log_n, m):
     perm, zeta = rng.randrange(P), rng.randrange(P)
     t = [rng.randrange(P) for _ in range(7 * nc * m - 9)]
     t_bl = [rng.randrange(P) for _ in range(7 * nc)]
-    srs = zk.SRS(ctx, G.cid, G.g[:m], G.mont_points(G.h_xy_canon)[0])
-    bufs = []
-    try:
-        got = device_ft(ctx, orc, fid, log_n, m, [(s6_8, perm)], t, zeta, bufs)
-        check_against_replay(orc, fid, log_n, m, [(s6_8, perm)], t, zeta, got)
-        coeffs, ft_len = got[0], got[1]
-        t_comm = srs.commit_custom(ev.mont(orc, fid, t), 7 * nc, ev.mont(orc, fid, t_bl)).chunks
-        s6_comm = srs.commit_non_hiding(ev.mont(orc, fid, s6), nc).chunks
-        assert t_comm.shape[0] == 7 * nc and s6_comm.shape[0] == nc
-        bft = fr.blinding_ft(t_bl, zeta, log_n, m, P)
-        mine = srs.commit_custom(coeffs[:ft_len], 1, ev.mont(orc, fid, [bft])).chunks
-        assert mine.shape[0] == 1
-        assert np.array_equal(mine[0], verifier_ft_comm(orc, G, s6_comm, t_comm, perm, zeta, log_n, m))
-    finally:
-        free_all(ctx, bufs)
-        srs.close()
+    with zk.SRS(ctx, G.cid, G.g[:m], G.mont_points(G.h_xy_canon)[0]) as srs:
+        with ctx.buffers() as bufs:
+            got = device_ft(ctx, orc, fid, log_n, m, [(s6_8, perm)], t, zeta, bufs)
+            check_against_replay(orc, fid, log_n, m, [(s6_8, perm)], t, zeta, got)
+            coeffs, ft_len = got[0], got[1]
+            t_comm = srs.commit_custom(ev.mont(orc, fid, t), 7 * nc, ev.mont(orc, fid, t_bl)).chunks
+            s6_comm = srs.commit_non_hiding(ev.mont(orc, fid, s6), nc).chunks
+            assert t_comm.shape[0] == 7 * nc and s6_comm.shape[0] == nc
+            bft = fr.blinding_ft(t_bl, zeta, log_n, m, P)
+            mine = srs.commit_custom(coeffs[:ft_len], 1, ev.mont(orc, fid, [bft])).chunks
+            assert mine.shape[0] == 1
+            assert np.array_equal(mine[0], verifier_ft_comm(orc, G, s6_comm, t_comm, perm, zeta, log_n, m))
 
 
 def test_one_proofs_tail_resident(ctx, orc, vesta_srs):
@@ -235,11 +209,10 @@ def test_one_proofs_tail_resident(ctx, orc, vesta_srs):
     h = G.mont_points(G.h_xy_canon)[0]
     srs = zk.SRS(ctx, cid, G.g[:m], h)
     bases = ctx.upload_bases(cid, G.g[:m])
-    bufs, lbs = [], []
-    try:
+    with srs, ctx.buffers() as bufs, contextlib.ExitStack() as stack:
         # 1. t = numerator / Z_H on the device
-        d_num = put(ctx, bufs, ev.mont(orc, fid, num))
-        d_t = ctx.dev_alloc(7 * n * 32); bufs.append(d_t)
+        d_num = bufs.put(ev.mont(orc, fid, num))
+        d_t = bufs.alloc(7 * n * 32)
         assert ctx.poly_divide_by_vanishing_dev(fid, d_num, 8 * n, log_n, d_t) is True
         # 2. t_comm: the 14 chunk MSMs on the resident t, masked with the blinders
         raw = np.stack([zk.jacobian_to_affine(cid, ctx.msm_dev(bases, d_t + c * m * 32, m, mont=True)) for c in range(7 * nc)])
@@ -247,14 +220,14 @@ def test_one_proofs_tail_resident(ctx, orc, vesta_srs):
         assert np.array_equal(t_comm, srs.commit_custom(ev.mont(orc, fid, q), 7 * nc, ev.mont(orc, fid, t_bl)).chunks)
         s6_comm = srs.commit_non_hiding(ev.mont(orc, fid, s6), nc).chunks
         # 3. evaluations at zeta and zeta omega
-        d_s8 = put(ctx, bufs, ev.mont(orc, fid, s6_8))
-        lbs = [zk.LagrangeBasisEvaluations(ctx, fid, m, log_n, m1(orc, fid, x)) for x in (zeta, zo)]
+        d_s8 = bufs.put(ev.mont(orc, fid, s6_8))
+        lbs = [stack.enter_context(zk.LagrangeBasisEvaluations(ctx, fid, m, log_n, m1(orc, fid, x))) for x in (zeta, zo)]
         s6_ev = ev.ints(orc, fid, zk.LagrangeBasisEvaluations.evaluate_all(lbs, [(d_s8, 8 * n, False)])[0])    # [point][chunk]
         s6_ev = [s6_ev[:nc], s6_ev[nc:]]
         t_ev = ev.ints(orc, fid, ctx.poly_evaluate_chunks_dev(fid, [(d_t, 7 * n)], 7 * nc, m, ev.mont(orc, fid, [zeta, zo]))[0])
         t_ev = [t_ev[:7 * nc], t_ev[7 * nc:]]
         # 4. ft
-        d_ft = ctx.dev_alloc(m * 32); bufs.append(d_ft)
+        d_ft = bufs.alloc(m * 32)
         ft_len, e1 = ctx.prover_ft_dev(fid, log_n, m, [(d_s8, 8 * n, m1(orc, fid, perm))], d_t, 7 * n, m1(orc, fid, zeta), d_ft)
         _, want, want_e1 = fr.ft(orc, fid, log_n, m, [(s6_8, perm)], q, zeta)
         assert ft_len == len(want) and np.array_equal(e1, m1(orc, fid, want_e1))
@@ -297,11 +270,6 @@ def test_one_proofs_tail_resident(ctx, orc, vesta_srs):
 
         assert verify(ft_eval1) is True
         assert verify((ft_eval1 + 1) % P) is False
-    finally:
-        for lb in lbs:
-            lb.close()
-        free_all(ctx, bufs)
-        srs.close()
 
 
 # ---------------------------------------------------------------------------------------------------------------- errors, threads
@@ -312,11 +280,10 @@ def test_errors_leave_ft_untouched(ctx, orc):
     rng = random.Random(3)
     z = m1(orc, fid, 5)
     bad = np.array([P & (2**64 - 1), (P >> 64) & (2**64 - 1), (P >> 128) & (2**64 - 1), P >> 192], dtype=np.uint64)
-    bufs = []
-    try:
-        d_e = put(ctx, bufs, ev.mont(orc, fid, [rng.randrange(P) for _ in range(8 * n)]))
-        d_t = put(ctx, bufs, ev.mont(orc, fid, [rng.randrange(P) for _ in range(7 * m + 1)]))
-        d_ft = put(ctx, bufs, stale(m))
+    with ctx.buffers() as bufs:
+        d_e = bufs.put(ev.mont(orc, fid, [rng.randrange(P) for _ in range(8 * n)]))
+        d_t = bufs.put(ev.mont(orc, fid, [rng.randrange(P) for _ in range(7 * m + 1)]))
+        d_ft = bufs.put(stale(m))
         good = [(d_e, 8 * n, z)]
         cases = [
             (-1, dict(field=7)), (-1, dict(log_n=31)), (-1, dict(mps=0)), (-1, dict(log_n=7, mps=48)),
@@ -345,8 +312,6 @@ def test_errors_leave_ft_untouched(ctx, orc):
         ln0, e0 = ctx.prover_ft_dev(fid, log_n, m, [], 0, 0, z, d_ft)
         assert ln0 == 0 and not e0.any() and not ctx.dev_download(d_ft, (m, 4)).any()
         assert ctx.prover_ft_dev(fid, log_n, m, good, d_t, 7 * m, z, d_ft)[0] > 0
-    finally:
-        free_all(ctx, bufs)
 
 
 def test_two_threads_share_a_context(ctx, orc):
@@ -360,11 +325,7 @@ def test_two_threads_share_a_context(ctx, orc):
         zeta = rng.randrange(P)
         _, want, want_e1 = fr.ft(orc, fid, log_n, m, terms, t, zeta)
         cases.append((terms, t, zeta, want, want_e1))
-    bufs, errors = [], []
-    dev = []
-    for terms, t, zeta, _, _ in cases:
-        d_terms = [(put(ctx, bufs, ev.mont(orc, fid, e)), len(e), m1(orc, fid, c)) for e, c in terms]
-        dev.append((d_terms, put(ctx, bufs, ev.mont(orc, fid, t)), put(ctx, bufs, stale(m))))
+    errors, dev = [], []
 
     def work(k):
         try:
@@ -378,12 +339,13 @@ def test_two_threads_share_a_context(ctx, orc):
         except Exception as e:                    # reported by the main thread
             errors.append(e)
 
-    try:
+    with ctx.buffers() as bufs:
+        for terms, t, zeta, _, _ in cases:
+            d_terms = [(bufs.put(ev.mont(orc, fid, e)), len(e), m1(orc, fid, c)) for e, c in terms]
+            dev.append((d_terms, bufs.put(ev.mont(orc, fid, t)), bufs.put(stale(m))))
         th = [threading.Thread(target=work, args=(k,)) for k in range(2)]
         for t in th:
             t.start()
         for t in th:
             t.join()
-    finally:
-        free_all(ctx, bufs)
     assert not errors, errors

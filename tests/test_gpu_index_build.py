@@ -75,8 +75,7 @@ def test_sections_match_the_restatement(ctx, orc, fid, log_n, zk_rows, n_gates, 
     endo = ev.mont(orc, fid, [12345])[0]
     kw = dict(public_inputs=3, prev_challenges=2, max_poly_size=1 << 16, feature_flags=0x41, lookup_selectors_present=0,
               disable_gates_checks=1, has_verifier_index_digest=1, endo=endo, verifier_index_digest=[1, 2, 3, 4], identifier=b"circuit-7")
-    idx = build(ctx, orc, fid, n, zk_rows, gates, shifts, optional, **kw)
-    try:
+    with build(ctx, orc, fid, n, zk_rows, gates, shifts, optional, **kw) as idx:
         want = ir.sections(orc, fid, n, zk_rows, gates, shifts, optional)
         h = idx.header
         assert h.num_sections == len(want) == 29 + bin(optional).count("1")
@@ -95,16 +94,13 @@ def test_sections_match_the_restatement(ctx, orc, fid, log_n, zk_rows, n_gates, 
             if not optional >> b & 1:
                 with pytest.raises(zk.ZkError):
                     idx.section(0x40 + b)
-    finally:
-        idx.close()
 
 
 @pytest.mark.parametrize("fid", [0, 1])
 def test_zero_selectors(ctx, orc, fid):
     n, zk_rows = 256, 4
     gates, shifts = circuit(orc, fid, n, 200, seed=5 + fid)
-    idx = build(ctx, orc, fid, n, zk_rows, gates, shifts, ALL_OPTIONAL, zero_selectors=True)
-    try:
+    with build(ctx, orc, fid, n, zk_rows, gates, shifts, ALL_OPTIONAL, zero_selectors=True) as idx:
         want = ir.sections(orc, fid, n, zk_rows, gates, shifts, ALL_OPTIONAL, zero_selectors=True)
         zeroed = set(ir.selector_tags(ALL_OPTIONAL))
         assert zeroed == {0x22, 0x23, 0x24, 0x25} | {0x40 + b for b in range(6)}
@@ -112,8 +108,6 @@ def test_zero_selectors(ctx, orc, fid):
             got, d = section(ctx, idx, tag)
             assert d == dom and np.array_equal(got, payload), hex(tag)
             assert (not got.any()) == (tag in zeroed), hex(tag)
-    finally:
-        idx.close()
 
 
 # ---------------------------------------------------------------------------------------------------------------- 3: built == loaded
@@ -131,22 +125,18 @@ def test_built_index_equals_the_loaded_file(ctx, orc, fid):
     n, zk_rows, optional = 512, 6, 0b001100
     gates, shifts = circuit(orc, fid, n, 300, seed=11 + fid)
     endo = ev.mont(orc, fid, [77])[0]
-    loaded = zk.IndexCache(ctx, cache_image(orc, fid, n, zk_rows, gates, shifts, optional, endo))
-    built = build(ctx, orc, fid, n, zk_rows, gates, shifts, optional, public_inputs=1, max_poly_size=n, endo=endo, identifier=b"vk")
-    try:
-        hb, hl = built.header, loaded.header
-        for f, _ in zk.IndexHeader._fields_:
-            if f not in ("num_sections", "shift", "endo", "verifier_index_digest"):
-                assert getattr(hb, f) == getattr(hl, f), f
-        assert [list(r) for r in hb.shift] == [list(r) for r in hl.shift] and list(hb.endo) == list(hl.endo)
-        assert hl.num_sections == hb.num_sections + 2                    # the file also holds the gates and their coefficients
-        for tag in [0x01] + ir.commitment_tags(optional):
-            a, da = section(ctx, built, tag)
-            b, db = section(ctx, loaded, tag)
-            assert da == db and np.array_equal(a, b), hex(tag)
-    finally:
-        built.close()
-        loaded.close()
+    with zk.IndexCache(ctx, cache_image(orc, fid, n, zk_rows, gates, shifts, optional, endo)) as loaded:
+        with build(ctx, orc, fid, n, zk_rows, gates, shifts, optional, public_inputs=1, max_poly_size=n, endo=endo, identifier=b"vk") as built:
+            hb, hl = built.header, loaded.header
+            for f, _ in zk.IndexHeader._fields_:
+                if f not in ("num_sections", "shift", "endo", "verifier_index_digest"):
+                    assert getattr(hb, f) == getattr(hl, f), f
+            assert [list(r) for r in hb.shift] == [list(r) for r in hl.shift] and list(hb.endo) == list(hl.endo)
+            assert hl.num_sections == hb.num_sections + 2                    # the file also holds the gates and their coefficients
+            for tag in [0x01] + ir.commitment_tags(optional):
+                a, da = section(ctx, built, tag)
+                b, db = section(ctx, loaded, tag)
+                assert da == db and np.array_equal(a, b), hex(tag)
 
 
 # ---------------------------------------------------------------------------------------------------------------- 4: 2^21 rows
@@ -185,28 +175,21 @@ def test_commitments(ctx, orc, pallas_srs, vesta_srs, curve, log_n, m):
     fid = orc.SCALAR_FIELD[golden.cid]
     n, zk_rows, optional = 1 << log_n, 5, 0b100101
     gates, shifts = circuit(orc, fid, n, min(n, 3000), seed=log_n + fid)
-    srs = srs_of(ctx, golden, m)
-    idx = build(ctx, orc, fid, n, zk_rows, gates, shifts, optional)
-    try:
-        got = srs.index_commitments(idx)
-        chunks = max(1, n // m)
-        assert got.shape == (28 + 3, chunks, 8)
-        cols = ir.columns_d1(orc, fid, n, zk_rows, gates, shifts, optional)
-        want = ir.commitments(orc, golden.cid, golden.g[:m], srs.h, cols, optional)
-        assert np.array_equal(got, want)
-        # the masked ones are h away from commit_evaluations_non_hiding
-        plain = srs.commit_evaluations_non_hiding(n, cols[0x21]).chunks
-        assert np.array_equal(got[23], np.stack([orc.affine_add(golden.cid, p, srs.h) for p in plain]))
-        if log_n == 10:          # a loaded cache of the same circuit commits to the same points
-            endo = ev.mont(orc, fid, [1])[0]
-            loaded = zk.IndexCache(ctx, cache_image(orc, fid, n, zk_rows, gates, shifts, optional, endo))
-            try:
-                assert np.array_equal(srs.index_commitments(loaded), got)
-            finally:
-                loaded.close()
-    finally:
-        idx.close()
-        srs.close()
+    with srs_of(ctx, golden, m) as srs:
+        with build(ctx, orc, fid, n, zk_rows, gates, shifts, optional) as idx:
+            got = srs.index_commitments(idx)
+            chunks = max(1, n // m)
+            assert got.shape == (28 + 3, chunks, 8)
+            cols = ir.columns_d1(orc, fid, n, zk_rows, gates, shifts, optional)
+            want = ir.commitments(orc, golden.cid, golden.g[:m], srs.h, cols, optional)
+            assert np.array_equal(got, want)
+            # the masked ones are h away from commit_evaluations_non_hiding
+            plain = srs.commit_evaluations_non_hiding(n, cols[0x21]).chunks
+            assert np.array_equal(got[23], np.stack([orc.affine_add(golden.cid, p, srs.h) for p in plain]))
+            if log_n == 10:          # a loaded cache of the same circuit commits to the same points
+                endo = ev.mont(orc, fid, [1])[0]
+                with zk.IndexCache(ctx, cache_image(orc, fid, n, zk_rows, gates, shifts, optional, endo)) as loaded:
+                    assert np.array_equal(srs.index_commitments(loaded), got)
 
 
 # ---------------------------------------------------------------------------------------------------------------- 6: the resident chain
@@ -242,38 +225,25 @@ def test_permutation_on_a_built_index(ctx, orc, fid, log_n, zk_rows):
     rng = random.Random(log_n)
     beta, gamma, alpha0, r0, r1 = (rng.randrange(1, P) for _ in range(5))
     mont = lambda xs: ev.mont(orc, fid, xs)
-    idx = build(ctx, orc, fid, n, zk_rows, gates, shifts)
-    bufs = []
-
-    def put(a):
-        a = np.ascontiguousarray(a, dtype=np.uint64)
-        p = ctx.dev_alloc(a.nbytes)
-        bufs.append(p)
-        ctx.dev_upload(p, a)
-        return p
-    try:
+    with build(ctx, orc, fid, n, zk_rows, gates, shifts) as idx, ctx.buffers() as bufs:
         d_s = [idx.section(0x30 + k)[0] for k in range(7)]
-        d_wev = put(np.concatenate([mont(w[k]) for k in range(7)]))
+        d_wev = bufs.put(np.concatenate([mont(w[k]) for k in range(7)]))
         d_w = [d_wev + k * n * 32 for k in range(7)]
-        d_z = put(np.zeros((n, 4), dtype=np.uint64))
+        d_z = bufs.put(np.zeros((n, 4), dtype=np.uint64))
         b, g, sh, rn = mont([beta])[0], mont([gamma])[0], mont(shifts), mont([r0, r1])
         assert ctx.perm_aggreg_dev(fid, log_n, zk_rows, d_w, d_s, m8, b, g, sh, rn, d_z) is True
         sigma = [ev.ints(orc, fid, c) for t, c in sorted(ir.columns_d1(orc, fid, n, zk_rows, gates, shifts).items()) if 0x30 <= t <= 0x36]
         _, z_coeffs, ok = pr.perm_aggreg(orc, fid, log_n, zk_rows, w, sigma, shifts, beta, gamma, [r0, r1])
         assert ok and np.array_equal(ctx.dev_download(d_z, (n, 4)), mont(z_coeffs))
-        d_wc, d_w8, d_z8, d_zk8, d_out = (put(np.zeros((k, 4), dtype=np.uint64)) for k in (7 * n, 7 * m8, m8, m8, m8))
+        d_wc, d_w8, d_z8, d_zk8, d_out = (bufs.put(np.zeros((k, 4), dtype=np.uint64)) for k in (7 * n, 7 * m8, m8, m8, m8))
         ctx.ntt_dev_oop(fid, d_wev, n, n, d_wc, log_n, batch=7, inverse=True)
         ctx.ntt_dev_oop(fid, d_wc, n, n, d_w8, log_n + 3, batch=7)
         ctx.ntt_dev_oop(fid, d_z, n, n, d_z8, log_n + 3)
-        d_zk = put(mont(vanishing_coeffs(orc, fid, log_n, zk_rows)))
+        d_zk = bufs.put(mont(vanishing_coeffs(orc, fid, log_n, zk_rows)))
         ctx.ntt_dev_oop(fid, d_zk, 4, 4, d_zk8, log_n + 3)
         ctx.perm_quotient_dev(fid, log_n + 3, [d_w8 + k * m8 * 32 for k in range(7)], d_z8, d_s, d_zk8, b, g, mont([alpha0])[0], sh, d_out)
         out = ctx.dev_download(d_out, (m8, 4))
         assert not out[::8].any() and out.any()
-    finally:
-        for p in bufs:
-            ctx.dev_free(p)
-        idx.close()
 
 
 @pytest.mark.parametrize("fid,log_n", [(0, 8), (1, 11)])
@@ -292,14 +262,10 @@ def test_generic_gates_on_a_built_index(ctx, orc, fid, log_n):
             w[3 * h + 2][j] = -(cl * l + cr * r + cm * l * r + cc) * pow(co, P - 2, P) % P
         gates.append((ir.GENERIC, [(j, k) for k in range(7)], c))
     shifts = [1] + [rng.randrange(2, P) for _ in range(6)]
-    idx = build(ctx, orc, fid, n, 3, gates, shifts)
-    bufs = []
-    try:
-        d_w1 = ctx.dev_alloc(15 * n * 32)
-        d_w8 = ctx.dev_alloc(15 * 8 * n * 32)
-        d_out = ctx.dev_alloc(4 * n * 32)
-        bufs += [d_w1, d_w8, d_out]
-        ctx.dev_upload(d_w1, np.concatenate([ev.mont(orc, fid, c) for c in w]))
+    with build(ctx, orc, fid, n, 3, gates, shifts) as idx, ctx.buffers() as bufs:
+        d_w1 = bufs.put(np.concatenate([ev.mont(orc, fid, c) for c in w]))
+        d_w8 = bufs.alloc(15 * 8 * n * 32)
+        d_out = bufs.alloc(4 * n * 32)
         ctx.ntt_dev(fid, d_w1, log_n, batch=15, inverse=True)
         ctx.ntt_dev_oop(fid, d_w1, n, n, d_w8, log_n + 3, batch=15)
         cols = [(d_w8 + k * 8 * n * 32, 8 * n, 8) for k in range(15)]
@@ -308,10 +274,6 @@ def test_generic_gates_on_a_built_index(ctx, orc, fid, log_n):
         gp.generic_gate(zk.ExprProgram(), alphas).evaluations(ctx, fid, cols, 4 * n, 4, d_out)
         out = ctx.dev_download(d_out, (4 * n, 4))
         assert not out[::4].any() and out.any()
-    finally:
-        for p in bufs:
-            ctx.dev_free(p)
-        idx.close()
 
 
 # ---------------------------------------------------------------------------------------------------------------- 7: refusals
@@ -370,18 +332,17 @@ def test_refusals(ctx, orc):
 def test_commitment_refusals(ctx, orc, vesta_srs):
     fid, n = 0, 64                                                             # Vesta's scalars: Fp
     gates, shifts = circuit(orc, fid, n, 10, seed=10)
-    srs = srs_of(ctx, vesta_srs, 1 << 10)
-    other = build(ctx, orc, 1, n, 3, gates, shifts)                            # over Fq
     endo = ev.mont(orc, fid, [1])[0]
     image = lambda secs, optional=0: write_cache("vk", {"public": 0, "prev_challenges": 0, "zk_rows": 3, "max_poly_size": n, "domain_d1_size": n,
                                                         "optional_selectors_present": optional, "endo_limbs": [int(x) for x in endo],
                                                         "shift_limbs": [[0] * 4] * 7}, secs)
     full = [(t, a.astype("<u8").tobytes(), d) for t, (a, d) in ir.sections(orc, fid, n, 3, gates, shifts).items()]
-    missing = zk.IndexCache(ctx, image([s for s in full if s[0] != 0x22]))
-    short = zk.IndexCache(ctx, image([s if s[0] != 0x24 else (0x24, s[1][:32 * 40], 0) for s in full]))
-    no_opt = zk.IndexCache(ctx, image(full, optional=0b10))
-    good = build(ctx, orc, fid, n, 3, gates, shifts)
-    try:
+    with (srs_of(ctx, vesta_srs, 1 << 10) as srs,
+          build(ctx, orc, 1, n, 3, gates, shifts) as other,                    # over Fq
+          zk.IndexCache(ctx, image([s for s in full if s[0] != 0x22])) as missing,
+          zk.IndexCache(ctx, image([s if s[0] != 0x24 else (0x24, s[1][:32 * 40], 0) for s in full])) as short,
+          zk.IndexCache(ctx, image(full, optional=0b10)) as no_opt,
+          build(ctx, orc, fid, n, 3, gates, shifts) as good):
         out = np.zeros((64, 8), dtype=np.uint64)
         k = ctypes.c_size_t()
         call = lambda idx, cap=64: zk.lib().zk_index_commitments(srs._h, idx._h if idx else None, out.ctypes.data_as(ctypes.POINTER(ctypes.c_uint64)), cap, ctypes.byref(k))
@@ -389,9 +350,6 @@ def test_commitment_refusals(ctx, orc, vesta_srs):
             assert call(idx) == -1, name
         assert call(good, cap=27) == -1 and k.value == 28
         assert call(good) == 0 and k.value == 28
-    finally:
-        for h in (other, missing, short, no_opt, good, srs):
-            h.close()
 
 
 # ---------------------------------------------------------------------------------------------------------------- 8: streams, threads
@@ -401,8 +359,7 @@ def test_on_a_callers_stream(orc, vesta_srs):
     gates, shifts = circuit(orc, fid, n, 4000, seed=12)
     want = ir.sections(orc, fid, n, zk_rows, gates, shifts, 0b1)
     stream = torch.cuda.Stream()
-    c = zk.Context(0)
-    try:
+    with zk.Context(0) as c:
         c.set_stream(stream.cuda_stream)
         srs = srs_of(c, vesta_srs, 1 << 16)
         srs.get_lagrange_basis_from_domain_size(n)
@@ -418,8 +375,6 @@ def test_on_a_callers_stream(orc, vesta_srs):
         assert np.array_equal(got, ir.commitments(orc, vesta_srs.cid, vesta_srs.g[:1 << 16], srs.h, cols, 0b1))
         idx.close()
         srs.close()
-    finally:
-        c.close()
 
 
 def test_two_threads_share_a_context(ctx, orc):

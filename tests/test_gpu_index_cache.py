@@ -39,8 +39,7 @@ def make_image(orc, fid, log_n, ident="vk-digest-abc", **kw):
 @pytest.mark.parametrize("fid", [0, 1])
 def test_sections_arrive_on_the_device_bit_for_bit(ctx, orc, fid):
     image, arrays, header = make_image(orc, fid, 8)
-    cache = zk.IndexCache(ctx, image, expect_identifier="vk-digest-abc")
-    try:
+    with zk.IndexCache(ctx, image, expect_identifier="vk-digest-abc") as cache:
         h = cache.header
         assert (h.public_inputs, h.prev_challenges, h.zk_rows, h.max_poly_size, h.domain_d1_size) == (3, 2, 3, 256, 256)
         assert h.identifier == b"vk-digest-abc" and h.feature_flags == 1 and h.num_sections == len(arrays) + 1
@@ -53,8 +52,6 @@ def test_sections_arrive_on_the_device_bit_for_bit(ctx, orc, fid):
             cache.section(0x02)                            # gates are not field elements
         with pytest.raises(zk.ZkError):
             cache.section(0x41)                            # optional selector not in this file
-    finally:
-        cache.close()
 
 
 def test_malformed_files_are_rejected(ctx, orc):
@@ -81,15 +78,8 @@ def test_cached_sigma_feeds_the_permutation_quotient(ctx, orc):
     shifts = np.array(header["shift_limbs"], dtype=np.uint64)
     sigma = np.stack([arrays[0x30 + i][0] for i in range(7)])
     want = orc.perm_quot(fid, w, z, sigma, zkpm, beta, gamma, alpha0, shifts)
-    cache = zk.IndexCache(ctx, image)
-    bufs = [ctx.dev_alloc(x.nbytes) for x in (w, z, zkpm, z)]
-    try:
-        for p, x in zip(bufs[:3], (w, z, zkpm)):
-            ctx.dev_upload(p, x)
+    with zk.IndexCache(ctx, image) as cache, ctx.buffers() as bufs:
+        d_w, d_z, d_zkpm, d_out = bufs.put(w), bufs.put(z), bufs.put(zkpm), bufs.alloc(z.nbytes)
         d_sigma = [cache.section(0x30 + i)[0] for i in range(7)]
-        ctx.perm_quotient_dev(fid, log_n + 3, [bufs[0] + k * m * 32 for k in range(7)], bufs[1], d_sigma, bufs[2], beta, gamma, alpha0, shifts, bufs[3])
-        assert np.array_equal(ctx.dev_download(bufs[3], (m, 4)), want)
-    finally:
-        for p in bufs:
-            ctx.dev_free(p)
-        cache.close()
+        ctx.perm_quotient_dev(fid, log_n + 3, [d_w + k * m * 32 for k in range(7)], d_z, d_sigma, d_zkpm, beta, gamma, alpha0, shifts, d_out)
+        assert np.array_equal(ctx.dev_download(d_out, (m, 4)), want)

@@ -152,9 +152,8 @@ def test_direct_base_fold_building_block(ctx, orc, request, name):
     g = G.g[: 2 * h].copy()
     g[3] = 0                      # identity in the low half
     g[h + 5] = 0                  # identity in the high half (the reference's zero padding, ipa.rs:848-850)
-    d_g, d_out = ctx.dev_alloc(g.nbytes), ctx.dev_alloc(g.nbytes // 2)
-    try:
-        ctx.dev_upload(d_g, g)
+    with ctx.buffers() as bufs:
+        d_g, d_out = bufs.put(g), bufs.alloc(g.nbytes // 2)
         for bits in (255, 128, 1):
             u = orc.limbs_to_ints(orc.random_scalars(G.scalar, 1, seed=bits))[0] % (1 << bits) or 1
             ctx.points_fold_dev(G.cid, d_g, h, orc.to_mont(G.scalar, orc.ints_to_limbs([u]))[0], d_out)
@@ -163,5 +162,3 @@ def test_direct_base_fold_building_block(ctx, orc, request, name):
                 hi = orc.scalar_mul(G.cid, g[h + i], u) if g[h + i].any() else np.zeros(8, dtype=np.uint64)
                 want = g[i] if not hi.any() else (hi if not g[i].any() else orc.affine_add(G.cid, g[i], hi))
                 assert np.array_equal(got[i], want), (bits, i)
-    finally:
-        ctx.dev_free(d_g); ctx.dev_free(d_out)

@@ -41,19 +41,6 @@ def canonical_ints(a) -> list:
     return [int.from_bytes(raw[k:k + 32], "little") for k in range(0, len(raw), 32)]
 
 
-def put(ctx, bufs, a):
-    a = np.ascontiguousarray(a, dtype=np.uint64)
-    p = ctx.dev_alloc(a.nbytes)
-    bufs.append(p)
-    ctx.dev_upload(p, a)
-    return p
-
-
-def free_all(ctx, bufs):
-    for p in bufs:
-        ctx.dev_free(p)
-
-
 # ---------------------------------------------------------------------------------------------------------------- three-pass NTT
 @pytest.mark.parametrize("fid,log_n", [(0, 21), (1, 23)])
 def test_coset_transforms(ctx, orc, fid, log_n):
@@ -74,11 +61,9 @@ def test_out_of_place_2_18_gates_to_d8(ctx, orc):
     fid, log_n, k = zk.FP, 18, 15
     n, m = 1 << log_n, 8 << log_n
     coeffs = rnd(orc, fid, k * n, 110).reshape(k, n, 4)
-    bufs = []
-    try:
-        d_c = put(ctx, bufs, coeffs)
-        d_8 = ctx.dev_alloc(k * m * 32)
-        bufs.append(d_8)
+    with ctx.buffers() as bufs:
+        d_c = bufs.put(coeffs)
+        d_8 = bufs.alloc(k * m * 32)
         pad = np.zeros((m, 4), dtype=np.uint64)
         for coset in (False, True):
             ctx.ntt_dev_oop(fid, d_c, n, n, d_8, log_n + 3, batch=k, coset=coset)
@@ -88,8 +73,6 @@ def test_out_of_place_2_18_gates_to_d8(ctx, orc):
                 pad[:n] = coeffs[j]
                 assert np.array_equal(got[j], orc.ntt(fid, pad, coset=coset)), (coset, j)
             del got
-    finally:
-        free_all(ctx, bufs)
 
 
 def test_in_place_batch_of_3_at_2_22(ctx, orc):
@@ -97,9 +80,8 @@ def test_in_place_batch_of_3_at_2_22(ctx, orc):
     fid, log_n, k = zk.FQ, 22, 3
     n = 1 << log_n
     a = rnd(orc, fid, k * n, 120).reshape(k, n, 4)
-    bufs = []
-    try:
-        d = put(ctx, bufs, a)
+    with ctx.buffers() as bufs:
+        d = bufs.put(a)
         ctx.ntt_dev(fid, d, log_n, batch=k)
         got = ctx.dev_download(d, (k, n, 4))
         for j in range(k):
@@ -107,8 +89,6 @@ def test_in_place_batch_of_3_at_2_22(ctx, orc):
         del got
         ctx.ntt_dev(fid, d, log_n, batch=k, inverse=True)
         assert np.array_equal(ctx.dev_download(d, (k, n, 4)), a)
-    finally:
-        free_all(ctx, bufs)
 
 
 def test_three_pass_sizes_build_no_full_table(ctx, orc):
@@ -159,11 +139,9 @@ def test_batches_beyond_the_grid_y_limit(ctx, orc):
     del got
     src = rnd(orc, fid, batch * 13, 141).reshape(batch, 13, 4)
     one = rnd(orc, fid, 65537 * 3, 142).reshape(65537, 3, 4)
-    bufs = []
-    try:
-        d_src, d_one = put(ctx, bufs, src), put(ctx, bufs, one)
-        d_out = ctx.dev_alloc(batch * n * 32)
-        bufs.append(d_out)
+    with ctx.buffers() as bufs:
+        d_src, d_one = bufs.put(src), bufs.put(one)
+        d_out = bufs.alloc(batch * n * 32)
         ctx.ntt_dev_oop(fid, d_src, 13, 5, d_out, 3, batch=batch)
         got = ctx.dev_download(d_out, (batch, n, 4))
         pad = np.zeros((n, 4), dtype=np.uint64)
@@ -172,8 +150,6 @@ def test_batches_beyond_the_grid_y_limit(ctx, orc):
             assert np.array_equal(got[j], orc.ntt(fid, pad)), j
         ctx.ntt_dev_oop(fid, d_one, 3, 1, d_out, 0, batch=65537)
         assert np.array_equal(ctx.dev_download(d_out, (65537, 4)), one[:, 0])
-    finally:
-        free_all(ctx, bufs)
 
 
 # ---------------------------------------------------------------------------------------------------------------- Lagrange basis
@@ -188,19 +164,15 @@ def test_lagrange_basis_and_evaluate_at_2_21(ctx, orc, fid, max_poly_size):
     col = orc.random_scalars(fid, n, seed=151 + fid)
     basis = ev.lagrange_basis(orc, fid, max_poly_size, log_n, x)
     want_eval = ev.mont(orc, fid, ev.evaluate(basis, canonical_ints(col), P))
-    bufs = []
-    lb = zk.LagrangeBasisEvaluations(ctx, fid, max_poly_size, log_n, ev.mont(orc, fid, [x])[0])
-    try:
-        assert lb.chunks == len(basis) == max(1, n // max_poly_size)
-        got = lb.evals()
-        for k, v in enumerate(basis):
-            assert np.array_equal(got[k], ev.mont(orc, fid, v)), k
-        del got
-        d_col = put(ctx, bufs, orc.to_mont(fid, col))
-        assert np.array_equal(lb.evaluate((d_col, n)), want_eval)
-    finally:
-        lb.close()
-        free_all(ctx, bufs)
+    with ctx.buffers() as bufs:
+        with zk.LagrangeBasisEvaluations(ctx, fid, max_poly_size, log_n, ev.mont(orc, fid, [x])[0]) as lb:
+            assert lb.chunks == len(basis) == max(1, n // max_poly_size)
+            got = lb.evals()
+            for k, v in enumerate(basis):
+                assert np.array_equal(got[k], ev.mont(orc, fid, v)), k
+            del got
+            d_col = bufs.put(orc.to_mont(fid, col))
+            assert np.array_equal(lb.evaluate((d_col, n)), want_eval)
 
 
 # ---------------------------------------------------------------------------------------------------------------- permutation
@@ -209,17 +181,13 @@ def device_z(ctx, orc, fid, log_n, zk_rows, w, sigma, beta, gamma, shifts, rand)
     -> (z's coefficients, final-value flag)"""
     n = 1 << log_n
     m = lambda xs: ev.mont(orc, fid, xs)
-    bufs = []
-    try:
-        d_w, d_s = put(ctx, bufs, w), put(ctx, bufs, sigma)
-        d_z = ctx.dev_alloc(n * 32)
-        bufs.append(d_z)
+    with ctx.buffers() as bufs:
+        d_w, d_s = bufs.put(w), bufs.put(sigma)
+        d_z = bufs.alloc(n * 32)
         ok = ctx.perm_aggreg_dev(fid, log_n, zk_rows, [d_w + k * n * 32 for k in range(7)],
                                  [d_s + k * sigma.shape[1] * 32 for k in range(7)], sigma.shape[1], m([beta])[0], m([gamma])[0],
                                  m(shifts), m(rand), d_z)
         return ctx.dev_download(d_z, (n, 4)), ok
-    finally:
-        free_all(ctx, bufs)
 
 
 def draw_scalars(P, seed):

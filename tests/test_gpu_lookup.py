@@ -30,26 +30,8 @@ def ctx():
     c.close()
 
 
-class Bufs:
-    """device buffers of one test, freed at the end"""
-
-    def __init__(self, ctx):
-        self.ctx, self.ptrs = ctx, []
-
-    def put(self, a):
-        a = np.ascontiguousarray(a, dtype=np.uint64)
-        p = self.ctx.dev_alloc(max(a.nbytes, 32))
-        self.ptrs.append(p)
-        if a.nbytes:
-            self.ctx.dev_upload(p, a)
-        return p
-
-    def stale(self, n):
-        return self.put(np.full((n, 4), STALE, dtype=np.uint64))
-
-    def free(self):
-        for p in self.ptrs:
-            self.ctx.dev_free(p)
+def stale(bufs, n):
+    return bufs.put(np.full((n, 4), STALE, dtype=np.uint64))
 
 
 def mont(orc, fid, xs):
@@ -83,9 +65,9 @@ def upload(orc, fid, inst, bufs, stride=1):
     return d_w, bufs.put(table_strided(orc, fid, inst.T1, stride, 5))
 
 
-def run_sorted(ctx, orc, fid, inst, d_w, d_t, stride, bufs, info=None):
+def run_sorted(ctx, orc, fid, inst, d_w, d_t, stride, bufs, info=None, d_s=None):
     n = inst.n
-    d_s = [bufs.stale(n) for _ in range(inst.m + 1)]
+    d_s = d_s or [stale(bufs, n) for _ in range(inst.m + 1)]
     row = ctx.lookup_sorted_dev(fid, n.bit_length() - 1, inst.zk_rows, d_w, d_t, stride, info or info_of(orc, fid, inst),
                                 mont(orc, fid, inst.rand_sorted), d_s)
     return row, d_s, [ctx.dev_download(p, (n, 4)) for p in d_s]
@@ -93,7 +75,7 @@ def run_sorted(ctx, orc, fid, inst, d_w, d_t, stride, bufs, info=None):
 
 def run_aggreg(ctx, orc, fid, inst, d_w, d_t, stride, d_s, bufs):
     n = inst.n
-    d_a = bufs.stale(n)
+    d_a = stale(bufs, n)
     b, g = mont(orc, fid, [inst.beta, inst.gamma])
     ok = ctx.lookup_aggreg_dev(fid, n.bit_length() - 1, inst.zk_rows, d_w, d_t, stride, info_of(orc, fid, inst), d_s, b, g,
                                mont(orc, fid, inst.rand_agg), d_a)
@@ -118,16 +100,13 @@ def test_joint_table(ctx, orc, fid, log_n, n_cols, ids, runtime):
     jc, tic = rng.randrange(P), rng.randrange(P)
     ints = lambda a: ev.ints(orc, fid, a)
     want = mont(orc, fid, lr.joint_table([ints(c) for c in cols], jc, tic, P, ints(tid8) if ids else None, ints(rt8) if runtime else None))
-    bufs = Bufs(ctx)
-    try:
+    with ctx.buffers() as bufs:
         d_c = [bufs.put(c) for c in cols]
-        d8, d1 = bufs.stale(m8), bufs.stale(m8 // 8)
+        d8, d1 = stale(bufs, m8), stale(bufs, m8 // 8)
         ctx.lookup_joint_table_dev(fid, log_n, d_c, *mont(orc, fid, [jc, tic]), d8, bufs.put(tid8) if ids else None,
                                    bufs.put(rt8) if runtime else None, d1)
         assert np.array_equal(ctx.dev_download(d8, (m8, 4)), want)
         assert np.array_equal(ctx.dev_download(d1, (m8 // 8, 4)), want[::8])
-    finally:
-        bufs.free()
 
 
 # ---------------------------------------------------------------------------------------------------------------- sorted + aggregation
@@ -145,8 +124,7 @@ def test_sorted_and_aggregation_match_the_reference(ctx, orc, fid, log_n, zk_row
     s = lr.sorted_patched(inst)
     agg, ok = lr.aggregation(inst, s)
     assert ok
-    bufs = Bufs(ctx)
-    try:
+    with ctx.buffers() as bufs:
         d_w, d_t = upload(orc, fid, inst, bufs, stride)
         row, d_s, got = run_sorted(ctx, orc, fid, inst, d_w, d_t, stride, bufs)
         assert row == -1
@@ -154,8 +132,6 @@ def test_sorted_and_aggregation_match_the_reference(ctx, orc, fid, log_n, zk_row
             assert np.array_equal(got[k], mont(orc, fid, s[k])), k
         dok, got_a = run_aggreg(ctx, orc, fid, inst, d_w, d_t, stride, d_s, bufs)
         assert dok is True and np.array_equal(got_a, mont(orc, fid, agg))
-    finally:
-        bufs.free()
 
 
 GATES = ["Xor16", "Lookup", "RangeCheck0", "RangeCheck1", "ForeignFieldMul", "Rot64", "Zero", "Generic"]
@@ -173,15 +149,12 @@ def test_kimchi_gates_and_one_hot_value(ctx, orc, fid, hot):
     inst = lr.instance(P, log_n, zk_rows, 4, seed=7 + fid, gates=gates, hot=hot)
     s = lr.sorted_patched(inst)
     agg, ok = lr.aggregation(inst, s)
-    bufs = Bufs(ctx)
-    try:
+    with ctx.buffers() as bufs:
         d_w, d_t = upload(orc, fid, inst, bufs, 8)
         row, d_s, got = run_sorted(ctx, orc, fid, inst, d_w, d_t, 8, bufs)
         assert row == -1 and all(np.array_equal(got[k], mont(orc, fid, s[k])) for k in range(5))
         dok, got_a = run_aggreg(ctx, orc, fid, inst, d_w, d_t, 8, d_s, bufs)
         assert ok and dok and np.array_equal(got_a, mont(orc, fid, agg))
-    finally:
-        bufs.free()
 
 
 @pytest.mark.parametrize("fid", [0, 1])
@@ -199,14 +172,11 @@ def test_missing_values_report_the_smallest_row_and_write_nothing(ctx, orc, fid)
         with pytest.raises(lr.ValueNotInTable) as e:
             lr.sorted_columns(inst)
         assert e.value.row == min(rows)
-        bufs = Bufs(ctx)
-        try:
+        with ctx.buffers() as bufs:
             d_w, d_t = upload(orc, fid, inst, bufs, 1)
             row, _, got = run_sorted(ctx, orc, fid, inst, d_w, d_t, 1, bufs)
             assert row == min(rows), case
             assert all(np.array_equal(g, s) for g, s in zip(got, stale_cols(m + 1, inst.n))), case
-        finally:
-            bufs.free()
 
 
 @pytest.mark.parametrize("fid", [0, 1])
@@ -218,16 +188,14 @@ def test_dummy_missing_while_padding_is_refused(ctx, orc, fid):
     inst.row_pattern = [p if i != 3 else 0 for i, p in enumerate(inst.row_pattern)]
     with pytest.raises(lr.Malformed):
         lr.sorted_columns(inst)
-    bufs = Bufs(ctx)
-    try:
+    with ctx.buffers() as bufs:
         d_w, d_t = upload(orc, fid, inst, bufs, 1)
+        d_s = [stale(bufs, inst.n) for _ in range(m + 1)]
         with pytest.raises(zk.ZkError) as e:
-            run_sorted(ctx, orc, fid, inst, d_w, d_t, 1, bufs)
+            run_sorted(ctx, orc, fid, inst, d_w, d_t, 1, bufs, d_s=d_s)
         assert e.value.code == -1 and "dummy" in str(e.value)
-        got = [ctx.dev_download(p, (inst.n, 4)) for p in bufs.ptrs[-(m + 1):]]
+        got = [ctx.dev_download(p, (inst.n, 4)) for p in d_s]
         assert all(np.array_equal(g, s) for g, s in zip(got, stale_cols(m + 1, inst.n)))
-    finally:
-        bufs.free()
 
 
 @pytest.mark.parametrize("fid", [0, 1])
@@ -248,8 +216,7 @@ def test_zero_denominators_and_a_perturbed_column(ctx, orc, fid):
     a, b = next((a, b) for a in range(L) for b in range(a + 1, L) if s[2][a] != s[2][b])
     s[2][a], s[2][b] = s[2][b], s[2][a]
     variants.append(("swapped", s))
-    bufs = Bufs(ctx)
-    try:
+    with ctx.buffers() as bufs:
         d_w, d_t = upload(orc, fid, inst, bufs, 1)
         for name, s in variants:
             want, ok = lr.aggregation(inst, s)
@@ -257,8 +224,6 @@ def test_zero_denominators_and_a_perturbed_column(ctx, orc, fid):
             dok, got = run_aggreg(ctx, orc, fid, inst, d_w, d_t, 1, d_s, bufs)
             assert dok == ok and not ok, name
             assert np.array_equal(got, mont(orc, fid, want)), name
-    finally:
-        bufs.free()
 
 
 # ---------------------------------------------------------------------------------------------------------------- the chain
@@ -291,31 +256,26 @@ def test_chain_from_an_index_cache_to_the_commitments(ctx, orc, pallas_srs):
                 [(0x50, np.concatenate([d8(c) for c in cols1]).astype("<u8").tobytes(), 8 * n), (0x51, d8(ids1).astype("<u8").tobytes(), 8 * n)])
     header = {"public": 0, "prev_challenges": 0, "zk_rows": zk_rows, "max_poly_size": n, "domain_d1_size": n, "lookup_selectors_present": 1,
               "endo_limbs": [0] * 4, "shift_limbs": [[0] * 4] * 7}
-    cache = zk.IndexCache(ctx, write_cache("lookup-chain", header, sections))
-    bufs = Bufs(ctx)
-    lag = G.lagrange_small(n)
-    bases = ctx.upload_bases(G.cid, lag)
-    try:
-        p50, n50, dom50 = cache.section(0x50)
-        p51, _, _ = cache.section(0x51)
-        assert n50 == 3 * 8 * n and dom50 == 8 * n
-        d_t8, d_t1 = bufs.stale(8 * n), bufs.stale(n)
-        ctx.lookup_joint_table_dev(fid, log_n, [p50 + k * 8 * n * 32 for k in range(3)], *mont(orc, fid, [inst.jc, inst.tic]), d_t8, p51, None, d_t1)
-        assert np.array_equal(ctx.dev_download(d_t1, (n, 4)), mont(orc, fid, T1))
-        d_w = [bufs.put(mont(orc, fid, c)) for c in inst.w]
-        row, d_s, got = run_sorted(ctx, orc, fid, inst, d_w, d_t8, 8, bufs)
-        assert row == -1 and all(np.array_equal(got[k], mont(orc, fid, s[k])) for k in range(m + 1))
-        d_a = bufs.stale(n)
-        b, g = mont(orc, fid, [inst.beta, inst.gamma])
-        assert ctx.lookup_aggreg_dev(fid, log_n, zk_rows, d_w, d_t8, 8, info_of(orc, fid, inst), d_s, b, g, mont(orc, fid, inst.rand_agg), d_a)
-        assert np.array_equal(ctx.dev_download(d_a, (n, 4)), mont(orc, fid, agg))
-        for k, (d, col) in enumerate(zip(d_s + [d_a], s + [agg])):
-            com = zk.jacobian_to_affine(G.cid, ctx.msm_dev(bases, d, n, mont=True))
-            assert np.array_equal(com, orc.msm_mont(G.cid, lag, mont(orc, fid, col))), k
-    finally:
-        bases.free()
-        bufs.free()
-        cache.close()
+    with zk.IndexCache(ctx, write_cache("lookup-chain", header, sections)) as cache:
+        with ctx.buffers() as bufs:
+            lag = G.lagrange_small(n)
+            with ctx.upload_bases(G.cid, lag) as bases:
+                p50, n50, dom50 = cache.section(0x50)
+                p51, _, _ = cache.section(0x51)
+                assert n50 == 3 * 8 * n and dom50 == 8 * n
+                d_t8, d_t1 = stale(bufs, 8 * n), stale(bufs, n)
+                ctx.lookup_joint_table_dev(fid, log_n, [p50 + k * 8 * n * 32 for k in range(3)], *mont(orc, fid, [inst.jc, inst.tic]), d_t8, p51, None, d_t1)
+                assert np.array_equal(ctx.dev_download(d_t1, (n, 4)), mont(orc, fid, T1))
+                d_w = [bufs.put(mont(orc, fid, c)) for c in inst.w]
+                row, d_s, got = run_sorted(ctx, orc, fid, inst, d_w, d_t8, 8, bufs)
+                assert row == -1 and all(np.array_equal(got[k], mont(orc, fid, s[k])) for k in range(m + 1))
+                d_a = stale(bufs, n)
+                b, g = mont(orc, fid, [inst.beta, inst.gamma])
+                assert ctx.lookup_aggreg_dev(fid, log_n, zk_rows, d_w, d_t8, 8, info_of(orc, fid, inst), d_s, b, g, mont(orc, fid, inst.rand_agg), d_a)
+                assert np.array_equal(ctx.dev_download(d_a, (n, 4)), mont(orc, fid, agg))
+                for k, (d, col) in enumerate(zip(d_s + [d_a], s + [agg])):
+                    com = zk.jacobian_to_affine(G.cid, ctx.msm_dev(bases, d, n, mont=True))
+                    assert np.array_equal(com, orc.msm_mont(G.cid, lag, mont(orc, fid, col))), k
 
 
 # ---------------------------------------------------------------------------------------------------------------- refusals
@@ -325,11 +285,10 @@ def test_refusals_leave_the_outputs_untouched(ctx, orc):
     inst = lr.instance(P, log_n, zk_rows, m, seed=90)
     L = inst.L
     bad = np.array([P & (2**64 - 1), (P >> 64) & (2**64 - 1), (P >> 128) & (2**64 - 1), P >> 192], dtype=np.uint64)
-    bufs = Bufs(ctx)
-    try:
+    with ctx.buffers() as bufs:
         d_w, d_t = upload(orc, fid, inst, bufs, 1)
-        d_s = [bufs.stale(n) for _ in range(m + 1)]
-        d_a = bufs.stale(n)
+        d_s = [stale(bufs, n) for _ in range(m + 1)]
+        d_a = stale(bufs, n)
         rs, ra = mont(orc, fid, inst.rand_sorted), mont(orc, fid, inst.rand_agg)
         b, g = mont(orc, fid, [inst.beta, inst.gamma])
         spec = spec_of(orc, fid, inst)
@@ -403,7 +362,7 @@ def test_refusals_leave_the_outputs_untouched(ctx, orc):
         # the joint table's refusals
         m8 = 8 * n
         cols = [bufs.put(orc.to_mont(fid, orc.random_scalars(fid, m8, seed=k))) for k in range(3)]
-        d8 = bufs.stale(m8)
+        d8 = stale(bufs, m8)
         jc, tic = sc[0], sc[1]
         for kw in [dict(field=7), dict(log_n=31), dict(cols=[]), dict(cols=cols[:1], rt=cols[1]), dict(jc=bad), dict(tic=bad), dict(out8=cols[2]),
                    dict(out8=cols[0] + 32 * 5), dict(out1=d8 + 32), dict(out1=cols[1]), dict(ids=d8)]:
@@ -417,17 +376,14 @@ def test_refusals_leave_the_outputs_untouched(ctx, orc):
         edge = lr.instance(P, log_n, n - 2, m, seed=91)
         row0, _, _ = run_sorted(ctx, orc, fid, edge, *upload(orc, fid, edge, bufs, 1), 1, bufs)
         assert row0 == -1
-    finally:
-        bufs.free()
 
 
 # ---------------------------------------------------------------------------------------------------------------- streams, threads
 def test_all_three_calls_on_a_callers_stream(orc):
     """inputs copied in behind a spin kernel on the caller's stream: any of the three calls running elsewhere reads zeros"""
     stream = torch.cuda.Stream()
-    c = zk.Context(0)
-    c.set_stream(stream.cuda_stream)
-    try:
+    with zk.Context(0) as c:
+        c.set_stream(stream.cuda_stream)
         fid, log_n, zk_rows, m = zk.FP, 10, 3, 4
         P, n = orc.MODULUS[fid], 1 << log_n
         inst = lr.instance(P, log_n, zk_rows, m, seed=100)
@@ -458,42 +414,35 @@ def test_all_three_calls_on_a_callers_stream(orc):
         for k in range(m + 1):
             assert np.array_equal(got[1 + k], mont(orc, fid, s[k])), k
         assert np.array_equal(got[-1], mont(orc, fid, agg))
-    finally:
-        c.close()
 
 
 def test_two_threads_share_a_context(ctx, orc):
     fid, log_n, zk_rows, m = zk.FQ, 11, 5, 4
     P, n = orc.MODULUS[fid], 1 << log_n
-    bufs, cases, errors = Bufs(ctx), [], []
-    for t in range(2):
-        inst = lr.instance(P, log_n, zk_rows, m - t, seed=200 + t)
-        s = lr.sorted_patched(inst)
-        agg, _ = lr.aggregation(inst, s)
-        d_w, d_t = upload(orc, fid, inst, bufs, 1)
-        cases.append((inst, d_w, d_t, s, agg))
+    cases, errors = [], []
 
     def work(t):
         try:
             inst, d_w, d_t, s, agg = cases[t]
-            mine = Bufs(ctx)
-            try:
+            with ctx.buffers() as mine:
                 for _ in range(4):
                     row, d_s, got = run_sorted(ctx, orc, fid, inst, d_w, d_t, 1, mine)
                     assert row == -1 and all(np.array_equal(got[k], mont(orc, fid, s[k])) for k in range(inst.m + 1))
                     ok, got_a = run_aggreg(ctx, orc, fid, inst, d_w, d_t, 1, d_s, mine)
                     assert ok and np.array_equal(got_a, mont(orc, fid, agg))
-            finally:
-                mine.free()
         except Exception as e:                    # reported by the main thread
             errors.append(e)
 
-    try:
+    with ctx.buffers() as bufs:
+        for t in range(2):
+            inst = lr.instance(P, log_n, zk_rows, m - t, seed=200 + t)
+            s = lr.sorted_patched(inst)
+            agg, _ = lr.aggregation(inst, s)
+            d_w, d_t = upload(orc, fid, inst, bufs, 1)
+            cases.append((inst, d_w, d_t, s, agg))
         th = [threading.Thread(target=work, args=(t,)) for t in range(2)]
         for t in th:
             t.start()
         for t in th:
             t.join()
-    finally:
-        bufs.free()
     assert not errors, errors

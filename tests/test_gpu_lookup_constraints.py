@@ -20,7 +20,7 @@ import lookup_constraints as lc
 import lookup_replay as lr
 import proof_systems_b200 as zk
 from index_cache_writer import write_cache
-from test_gpu_lookup import CASES, GATES, Bufs, info_of, mont
+from test_gpu_lookup import CASES, GATES, info_of, mont, stale
 
 pytestmark = pytest.mark.gpu
 
@@ -39,7 +39,7 @@ def lit_of(orc, fid):
 def to_d8(ctx, fid, log_n, d1, k, bufs):
     """k contiguous d1 columns -> k contiguous d8 columns: iFFT(n), then FFT(8n) with in_len = n"""
     n = 1 << log_n
-    coef, out = bufs.stale(k * n), bufs.stale(k * 8 * n)
+    coef, out = stale(bufs, k * n), stale(bufs, k * 8 * n)
     ctx.ntt_dev_oop(fid, d1, n, n, coef, log_n, batch=k, inverse=True)
     ctx.ntt_dev_oop(fid, coef, n, n, out, log_n + 3, batch=k)
     return out
@@ -61,7 +61,7 @@ def run(ctx, orc, fid, inst, bufs, patterns=None, table8=None, selectors8=None, 
     tic = inst.tic if device_tic is None else device_tic
     info = info_of(orc, fid, inst)
     info.table_id_combiner[:] = [int(x) for x in mont(orc, fid, [tic])[0]]
-    sa1 = bufs.stale((m + 2) * n)
+    sa1 = stale(bufs, (m + 2) * n)
     d_s = [sa1 + k * n * B for k in range(m + 1)]
     d_a = sa1 + (m + 1) * n * B
     assert ctx.lookup_sorted_dev(fid, log_n, inst.zk_rows, d_w, table8, 8, info, mont(orc, fid, inst.rand_sorted), d_s) == -1
@@ -89,7 +89,7 @@ def run(ctx, orc, fid, inst, bufs, patterns=None, table8=None, selectors8=None, 
     # each entry into its own buffer, and alpha-scaled into t8
     alphas = [random.Random(n + fid).randrange(1, P) for _ in lc.ENTRIES]
     scaled = lc.constraints(zk.ExprProgram, cfg)
-    d_e, d_t8 = [bufs.stale(m8) for _ in lc.ENTRIES], bufs.put(np.zeros((m8, 4), dtype=np.uint64))
+    d_e, d_t8 = [stale(bufs, m8) for _ in lc.ENTRIES], bufs.put(np.zeros((m8, 4), dtype=np.uint64))
     for prog, sp, a, d in zip(lc.constraints(zk.ExprProgram, cfg), scaled, alphas, d_e):
         prog.evaluations(ctx, fid, cols, m8, 8, d)
         sp.literal(mont(orc, fid, [a])[0]).mul().evaluations(ctx, fid, cols, m8, 8, d_t8, accumulate=True)
@@ -108,7 +108,7 @@ def run(ctx, orc, fid, inst, bufs, patterns=None, table8=None, selectors8=None, 
     assert np.array_equal(got_t8, orc.expr_eval(fid, comb.ops, comb.args, comb.literals, [(e, 1) for e in want], m8))
     bad_rows = [r for r in range(n) if got[0][8 * r].any()]
     # iFFT(8n), then the division by Z_H on the device
-    d_q = bufs.stale(m8)
+    d_q = stale(bufs, m8)
     div = []
     for d in d_e + [d_t8]:
         ctx.ntt_dev(fid, d, log_n + 3, inverse=True)
@@ -130,11 +130,8 @@ def test_the_device_lookup_argument_satisfies_the_constraints(ctx, orc, fid, log
     """stride 8: the lookup calls read the table from its d8 evaluations, as the prover's lookup_table8; stride 1 cases do too
     here, since the constraints need the table over d8 anyway"""
     inst = lr.instance(orc.MODULUS[fid], log_n, zk_rows, m, seed=1000 * fid + 10 * log_n + m, dummy_at=where, tic="kimchi")
-    bufs = Bufs(ctx)
-    try:
+    with ctx.buffers() as bufs:
         check_honest(run(ctx, orc, fid, inst, bufs))
-    finally:
-        bufs.free()
 
 
 @pytest.mark.parametrize("fid", [0, 1])
@@ -146,11 +143,8 @@ def test_kimchi_gates_and_one_hot_value(ctx, orc, fid, log_n, hot):
     rng = random.Random(fid + log_n)
     gates = ["RangeCheck0"] * L if hot else [rng.choice(GATES) for _ in range(L)]
     inst = lr.instance(P, log_n, zk_rows, 4, seed=7 + fid + log_n, gates=gates, hot=hot, tic="kimchi")
-    bufs = Bufs(ctx)
-    try:
+    with ctx.buffers() as bufs:
         check_honest(run(ctx, orc, fid, inst, bufs))
-    finally:
-        bufs.free()
 
 
 def test_no_table_ids(ctx, orc):
@@ -165,11 +159,8 @@ def test_no_table_ids(ctx, orc):
     table += [(lr.XOR_TABLE_ID, [0, 0, 0])] * 9
     inst = lr.instance(P, log_n, zk_rows, m, seed=31, gates=["Xor16"] * L, table=table, tic=0)
     assert inst.tic == 0 and any(inst.row_pattern)
-    bufs = Bufs(ctx)
-    try:
+    with ctx.buffers() as bufs:
         check_honest(run(ctx, orc, fid, inst, bufs, device_tic=0))
-    finally:
-        bufs.free()
 
 
 def test_chain_from_an_index_cache(ctx, orc, pallas_srs):
@@ -194,24 +185,20 @@ def test_chain_from_an_index_cache(ctx, orc, pallas_srs):
                 [(0x52 + k, d8(sel1[k]), 8 * n) for k in range(4)])
     header = {"public": 0, "prev_challenges": 0, "zk_rows": zk_rows, "max_poly_size": n, "domain_d1_size": n,
               "lookup_selectors_present": 0x1F, "endo_limbs": [0] * 4, "shift_limbs": [[0] * 4] * 7}
-    cache = zk.IndexCache(ctx, write_cache("lookup-constraints", header, sections))
-    bufs = Bufs(ctx)
-    try:
-        p50, _, _ = cache.section(0x50)
-        p51, _, _ = cache.section(0x51)
-        sel8 = []
-        for k in range(4):
-            p, cnt, dom = cache.section(0x52 + k)
-            assert cnt == 8 * n and dom == 8 * n
-            sel8.append(p)
-        d_t8, d_t1 = bufs.stale(8 * n), bufs.stale(n)
-        ctx.lookup_joint_table_dev(fid, log_n, [p50 + k * 8 * n * 32 for k in range(3)], *mont(orc, fid, [inst.jc, inst.tic]), d_t8, p51,
-                                   None, d_t1)
-        inst.T1 = ev.ints(orc, fid, ctx.dev_download(d_t1, (n, 4)))
-        check_honest(run(ctx, orc, fid, inst, bufs, patterns=kimchi, table8=d_t8, selectors8=sel8))
-    finally:
-        bufs.free()
-        cache.close()
+    with zk.IndexCache(ctx, write_cache("lookup-constraints", header, sections)) as cache:
+        with ctx.buffers() as bufs:
+            p50, _, _ = cache.section(0x50)
+            p51, _, _ = cache.section(0x51)
+            sel8 = []
+            for k in range(4):
+                p, cnt, dom = cache.section(0x52 + k)
+                assert cnt == 8 * n and dom == 8 * n
+                sel8.append(p)
+            d_t8, d_t1 = stale(bufs, 8 * n), stale(bufs, n)
+            ctx.lookup_joint_table_dev(fid, log_n, [p50 + k * 8 * n * 32 for k in range(3)], *mont(orc, fid, [inst.jc, inst.tic]), d_t8, p51,
+                                       None, d_t1)
+            inst.T1 = ev.ints(orc, fid, ctx.dev_download(d_t1, (n, 4)))
+            check_honest(run(ctx, orc, fid, inst, bufs, patterns=kimchi, table8=d_t8, selectors8=sel8))
 
 
 # ---------------------------------------------------------------------------------------------------------------- negative cases
@@ -220,11 +207,8 @@ def test_chain_from_an_index_cache(ctx, orc, pallas_srs):
 def test_each_perturbation_fails_exactly_its_constraints(ctx, orc, fid, kind):
     inst = lr.instance(orc.MODULUS[fid], 10, 5, 4, seed=600 + fid, tic="kimchi")
     must_fail, verdict = lc.NEGATIVE[kind]
-    bufs = Bufs(ctx)
-    try:
+    with ctx.buffers() as bufs:
         div, div_t8, final_is_one, got_verdict, bad_rows, row = run(ctx, orc, fid, inst, bufs, kind=kind)
-    finally:
-        bufs.free()
     assert {e for e, d in zip(lc.ENTRIES, div) if not d} == must_fail
     assert not div_t8 and got_verdict == verdict
     assert bad_rows == ([] if row is None else [row])

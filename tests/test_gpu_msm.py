@@ -139,12 +139,9 @@ def test_random_and_all_ones_scalars_vs_oracle(ctx, orc, vesta_srs, wb):
     n = 3000
     sc = orc.random_scalars(srs.scalar, n, seed=77)
     ones = np.zeros((n, 4), dtype=np.uint64); ones[:, 0] = 1
-    bases = ctx.upload_bases(srs.cid, srs.g[:n], window_bits=wb)
-    try:
+    with ctx.upload_bases(srs.cid, srs.g[:n], window_bits=wb) as bases:
         for scal in (sc, ones):
             assert np.array_equal(ctx.msm_affine(bases, scal), orc.msm(srs.cid, srs.g[:n], scal))
-    finally:
-        bases.free()
 
 
 def test_config2_2_16_pallas(ctx, orc, pallas_srs):

@@ -87,8 +87,7 @@ def test_finish_variant_x_chunk_x_log_g(ctx, orc, pallas_srs, sms, variant, chun
     g[n // 3] = 0
     sc = orc.limbs_to_ints(orc.random_scalars(srs.scalar, n, seed=n + chunk))
     sc[1:40] = [1] * 39                       # one heavier bucket: more than one task at the small chunks
-    bases = ctx.upload_bases(srs.cid, g, window_bits=wb)
-    try:
+    with ctx.upload_bases(srs.cid, g, window_bits=wb) as bases:
         p = mp.plan(n, 1, bases.window_bits, window, sms, chunk, wave)
         assert p.many_buckets == variant.startswith("serial") and p.capacity == sms * (wave or 512)
         if chunk:
@@ -100,8 +99,6 @@ def test_finish_variant_x_chunk_x_log_g(ctx, orc, pallas_srs, sms, variant, chun
             assert r.tasks == int(mp.buckets([sc], p).sum()) and r.multi > 0   # every entry a task
         with options(ctx, chunk, wave):
             run(ctx, orc, srs, bases, g, sc, p, window_bits=window)
-    finally:
-        bases.free()
 
 
 def test_log_g_takes_every_value_in_both_finish_variants():
@@ -114,8 +111,7 @@ def test_launch_count_tells_the_finish_variant(ctx, orc, pallas_srs, sms):
     srs = pallas_srs
     n = 500
     sc = orc.random_scalars(srs.scalar, n, seed=8)
-    bases = ctx.upload_bases(srs.cid, srs.g[:n], window_bits=0)
-    try:
+    with ctx.upload_bases(srs.cid, srs.g[:n], window_bits=0) as bases:
         delta = {}
         for window in (8, 10):
             before = ctx.launch_count
@@ -124,8 +120,6 @@ def test_launch_count_tells_the_finish_variant(ctx, orc, pallas_srs, sms):
         quad, serial = mp.plan(n, 1, 0, 8, sms), mp.plan(n, 1, 0, 10, sms)
         assert not quad.many_buckets and serial.many_buckets
         assert delta[10] - delta[8] == 1 and (delta[8], delta[10]) == (quad.launches, serial.launches)
-    finally:
-        bases.free()
 
 
 # ------------------------------------------------------------------------------------------ b. bucket populations at the boundaries
@@ -223,12 +217,9 @@ def test_bucket_populations_at_the_boundaries(ctx, orc, pallas_srs, sms, wb, chu
     assert [(b, int(counts[b])) for b in np.flatnonzero(counts)] == lay
     check_boundary_facts(lay, p, mp.regime(counts, p), giant_at)
     g = srs.g[:len(sc)]
-    bases = ctx.upload_bases(srs.cid, g, window_bits=wb)
-    try:
+    with ctx.upload_bases(srs.cid, g, window_bits=wb) as bases:
         with options(ctx, chunk):
             run(ctx, orc, srs, bases, g, sc, p)
-    finally:
-        bases.free()
 
 
 @pytest.mark.parametrize("entries", [1, 5, 3000])
@@ -236,8 +227,7 @@ def test_bucket_populations_at_the_boundaries(ctx, orc, pallas_srs, sms, wb, chu
 def test_a_single_populated_bucket(ctx, orc, vesta_srs, sms, wb, entries):
     srs = vesta_srs
     g = srs.g[:entries]
-    bases = ctx.upload_bases(srs.cid, g, window_bits=wb)
-    try:
+    with ctx.upload_bases(srs.cid, g, window_bits=wb) as bases:
         for digit in (1, 1234, 1 << (wb - 1)):
             sc = [digit] * entries
             p = mp.plan(entries, 1, wb, 0, sms, 1)
@@ -245,8 +235,6 @@ def test_a_single_populated_bucket(ctx, orc, vesta_srs, sms, wb, entries):
             assert r.empty == p.NB - 1 and r.s_b[digit - 1] == entries and len(r.giants) == (entries > p.smax)
             with options(ctx, 1):
                 run(ctx, orc, srs, bases, g, sc, p)
-    finally:
-        bases.free()
 
 
 # ------------------------------------------------------------------------------------------ c. how many giants
@@ -277,12 +265,9 @@ def test_number_of_giant_buckets(ctx, orc, vesta_srs, sms, wb, count):
     r = mp.regime(mp.buckets([sc], p), p)
     assert len(r.giants) == count and r.overflow == (count > 64) and p.many_buckets == (wb == 16) and r.multi >= 1 and r.single >= 1
     g = srs.g[:p.n]
-    bases = ctx.upload_bases(srs.cid, g, window_bits=wb)
-    try:
+    with ctx.upload_bases(srs.cid, g, window_bits=wb) as bases:
         with options(ctx, 1):
             run(ctx, orc, srs, bases, g, sc, p)
-    finally:
-        bases.free()
 
 
 @pytest.mark.parametrize("per_msm", [(0, 1, 20, 30), (0, 1, 30, 40)], ids=["51-giants", "71-giants-overflow"])
@@ -299,12 +284,9 @@ def test_giants_spread_over_the_groups_of_a_fused_batch(ctx, orc, vesta_srs, sms
     assert [int(np.sum(r.giants // p.B == j)) for j in range(p.k)] == list(per_msm) and r.overflow == (sum(per_msm) > 64)
     assert p.many_buckets == (wb == 16) and p.ntiles == (32 if wb == 16 else 1)
     g = srs.g[:p.n]
-    bases = ctx.upload_bases(srs.cid, g, window_bits=wb)
-    try:
+    with ctx.upload_bases(srs.cid, g, window_bits=wb) as bases:
         with options(ctx, 1):
             run(ctx, orc, srs, bases, g, sc, p)
-    finally:
-        bases.free()
 
 
 @pytest.mark.parametrize("count", [3, 70])
@@ -320,12 +302,9 @@ def test_giants_spread_over_the_windows_of_a_plain_run(ctx, orc, pallas_srs, sms
     r = mp.regime(mp.buckets([sc], p), p)
     assert len(r.giants) >= count and r.overflow == (count > 64) and len(set(r.giants // p.B)) > 2 and p.many_buckets == (window == 10)
     g = srs.g[:p.n]
-    bases = ctx.upload_bases(srs.cid, g, window_bits=0)
-    try:
+    with ctx.upload_bases(srs.cid, g, window_bits=0) as bases:
         with options(ctx, 1):
             run(ctx, orc, srs, bases, g, sc, p, window_bits=window)
-    finally:
-        bases.free()
 
 
 @pytest.mark.parametrize("wb", [16, 10], ids=["serial-table16", "quad-table10"])
@@ -336,16 +315,13 @@ def test_giant_list_starts_clean_after_an_overflow(ctx, orc, vesta_srs, sms, wb)
     cases = {}
     for count in (65, 1, 0):
         cases[count] = consistent(lambda p: giants_scalars(p, count), lambda n: mp.plan(n, 1, wb, 0, sms, 1))
-    bases = ctx.upload_bases(srs.cid, srs.g[:max(p.n for _, p in cases.values())], window_bits=wb)
-    try:
+    with ctx.upload_bases(srs.cid, srs.g[:max(p.n for _, p in cases.values())], window_bits=wb) as bases:
         with options(ctx, 1):
             for count in (65, 1, 0, 1, 65):
                 sc, p = cases[count]
                 r = mp.regime(mp.buckets([sc], p), p)
                 assert len(r.giants) == count and r.overflow == (count == 65)
                 run(ctx, orc, srs, bases, srs.g, sc, p)
-    finally:
-        bases.free()
 
 
 # ------------------------------------------------------------------------------------------ d. coinciding partials and buckets
@@ -395,12 +371,9 @@ def test_coinciding_partials_and_buckets(ctx, orc, pallas_srs, sms, wb, chunk):
     assert list(r.s_b[:10]) == [2, 2, 2 // chunk, 4, 1, 4, 3, 1, 1024, 1200] and list(r.giants) == [8, 9] and 1024 > p.smax
     # the two P, P, -P, -P buckets cross a boundary of k_run_sum's runs of 4 at different places
     assert r.task_off[3] % 4 != 0 and r.task_off[5] % 4 != 0 and r.task_off[3] % 4 != r.task_off[5] % 4
-    bases = ctx.upload_bases(srs.cid, g, window_bits=wb)
-    try:
+    with ctx.upload_bases(srs.cid, g, window_bits=wb) as bases:
         with options(ctx, chunk):
             run(ctx, orc, srs, bases, g, sc, p)
-    finally:
-        bases.free()
 
 
 @pytest.mark.parametrize("wb,window", [(16, 0), (10, 0), (0, 9)], ids=["serial-table16", "quad-table10", "plain9"])
@@ -411,8 +384,7 @@ def test_groups_that_sum_to_the_identity(ctx, orc, vesta_srs, sms, wb, window):
     g = np.concatenate([srs.g[:m], negated(orc, srs, srs.g[:m])])
     c = wb or window
     half = orc.limbs_to_ints(orc.random_scalars(srs.scalar, m, seed=5))
-    bases = ctx.upload_bases(srs.cid, g, window_bits=wb)
-    try:
+    with ctx.upload_bases(srs.cid, g, window_bits=wb) as bases:
         for chunk in (1, 2):
             p = mp.plan(2 * m, 1, wb, window, sms, chunk)
             with options(ctx, chunk):
@@ -424,8 +396,6 @@ def test_groups_that_sum_to_the_identity(ctx, orc, vesta_srs, sms, wb, window):
                     counts = mp.buckets([mixed], p)
                     assert counts[2 * p.B:3 * p.B].sum() > 0
                     run(ctx, orc, srs, bases, g, mixed, p, window_bits=window)
-    finally:
-        bases.free()
 
 
 # ------------------------------------------------------------------------------------------ e. tables and windows
@@ -442,8 +412,7 @@ def test_every_window_with_and_without_a_table(ctx, orc, pallas_srs, sms, c, tab
     sc = orc.random_scalars(srs.scalar, N, seed=c)
     sc[3] = orc.int_to_limbs(orc.MODULUS[srs.scalar] - 1)
     sc[4] = orc.int_to_limbs((1 << (c - 1)) + 1)
-    bases = ctx.upload_bases(srs.cid, g, window_bits=c if table else 0)
-    try:
+    with ctx.upload_bases(srs.cid, g, window_bits=c if table else 0) as bases:
         assert bases.window_bits == (c if table else 0)
         for n in (1, 31, 33, 127, 129, 1000):
             p = mp.plan(n, 1, bases.window_bits, c, sms)
@@ -453,8 +422,6 @@ def test_every_window_with_and_without_a_table(ctx, orc, pallas_srs, sms, c, tab
         run(ctx, orc, srs, bases, g, orc.limbs_to_ints(sc[:n]), p, window_bits=0 if table else c, off=off)
         mont = orc.to_mont(srs.scalar, sc[:n])
         assert np.array_equal(ctx.msm_affine(bases, mont, off=off, mont=True, window_bits=0 if table else c), orc.msm(srs.cid, g[off:off + n], sc[:n]))
-    finally:
-        bases.free()
 
 
 # ------------------------------------------------------------------------------------------ f. gathered partials
@@ -481,13 +448,10 @@ def test_gathered_partials_of_equal_slices(ctx, orc, vesta_srs, sms, wb, window,
     n = world * m
     sc = orc.random_scalars(srs.scalar, n, seed=world)
     d_sc = torch.from_numpy(sc.view(np.int64)).cuda()
-    bases = ctx.upload_bases(srs.cid, srs.g[:n], window_bits=wb)
-    try:
+    with ctx.upload_bases(srs.cid, srs.g[:n], window_bits=wb) as bases:
         p = mp.plan(m, 1, bases.window_bits, window, sms)
         got = gathered(ctx, orc, srs, bases, d_sc, [(r * m, r * m, m) for r in range(world)], window, p)
         assert np.array_equal(got, orc.msm(srs.cid, srs.g[:n], sc))
-    finally:
-        bases.free()
 
 
 @pytest.mark.parametrize("wb,window", [(9, 0), (0, 7)], ids=["table9", "plain7"])
@@ -502,14 +466,11 @@ def test_gathered_partials_that_coincide(ctx, orc, vesta_srs, sms, wb, window):
     A, NEG, ZERO = (0, 0, m), (m, 0, m), (0, m, m)
     want = {1: orc.msm(srs.cid, g[:m], sc[:m]), 2: orc.msm(srs.cid, np.concatenate([g[:m], g[:m]]), np.concatenate([sc[:m], sc[:m]])),
             0: np.zeros(8, dtype=np.uint64)}
-    bases = ctx.upload_bases(srs.cid, g, window_bits=wb)
-    try:
+    with ctx.upload_bases(srs.cid, g, window_bits=wb) as bases:
         p = mp.plan(m, 1, bases.window_bits, window, sms)
         for slices, mult in (([A, A], 2), ([A, NEG], 0), ([A, ZERO], 1), ([ZERO, A, A, NEG], 1), ([ZERO, ZERO, ZERO], 0),
                              ([A, A, NEG, NEG, A, ZERO, NEG, A, A, NEG], 1)):
             assert np.array_equal(gathered(ctx, orc, srs, bases, d_sc, slices, window, p), want[mult]), (slices, mult)
-    finally:
-        bases.free()
 
 
 # ------------------------------------------------------------------------------------------ g. workspace reuse
@@ -520,8 +481,7 @@ def test_workspace_reuse_across_shapes(orc, pallas_srs, sms):
     srs = pallas_srs
     n = 2048
     g = srs.g[:n]
-    ctx = zk.Context(0)
-    try:
+    with zk.Context(0) as ctx:
         plain = ctx.upload_bases(srs.cid, g, window_bits=0)
         t16 = ctx.upload_bases(srs.cid, g, window_bits=16)
         t10 = ctx.upload_bases(srs.cid, g, window_bits=10)
@@ -536,5 +496,3 @@ def test_workspace_reuse_across_shapes(orc, pallas_srs, sms):
             assert p.ntiles == ntiles
             with options(ctx, chunk):
                 run(ctx, orc, srs, bases, g, sc, p, window_bits=window)
-    finally:
-        ctx.close()

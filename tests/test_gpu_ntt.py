@@ -169,10 +169,8 @@ def test_out_of_place_device_pipeline(ctx, orc):
     fid, log_n, k = zk.FP, 10, 5
     n, m = 1 << log_n, 8 << log_n
     ev = orc.to_mont(fid, orc.random_scalars(fid, k * n, seed=90)).reshape(k, n, 4)
-    d_w = ctx.dev_alloc(ev.nbytes)
-    d_8 = ctx.dev_alloc(k * m * 32)
-    try:
-        ctx.dev_upload(d_w, ev)
+    with ctx.buffers() as bufs:
+        d_w, d_8 = bufs.put(ev), bufs.alloc(k * m * 32)
         ctx.ntt_dev(fid, d_w, log_n, batch=k, inverse=True)
         coeffs = ctx.dev_download(d_w, (k, n, 4))
         ctx.ntt_dev_oop(fid, d_w, n, n, d_8, log_n + 3, batch=k)
@@ -193,6 +191,3 @@ def test_out_of_place_device_pipeline(ctx, orc):
         pad[:n] = coeffs[2]
         assert np.array_equal(got2[2], orc.ntt(fid, pad, coset=True))
         assert np.array_equal(ctx.dev_download(d_w, (k, n, 4)), coeffs)
-    finally:
-        ctx.dev_free(d_w)
-        ctx.dev_free(d_8)

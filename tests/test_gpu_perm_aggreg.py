@@ -24,20 +24,6 @@ def ctx():
     c.close()
 
 
-def put(ctx, bufs, a):
-    a = np.ascontiguousarray(a, dtype=np.uint64)
-    p = ctx.dev_alloc(max(a.nbytes, 32))
-    bufs.append(p)
-    if a.nbytes:
-        ctx.dev_upload(p, a)
-    return p
-
-
-def free_all(ctx, bufs):
-    for p in bufs:
-        ctx.dev_free(p)
-
-
 def stale(n):
     """a recognisable pattern for d_z before a call"""
     return np.full((n, 4), 0x0123456789abcdef, dtype=np.uint64)
@@ -48,16 +34,16 @@ def scalars(orc, fid, inst):
     return m([inst.beta])[0], m([inst.gamma])[0], m(inst.shifts), m(inst.rand)
 
 
-def upload(ctx, orc, fid, inst, stride, bufs, seed):
+def upload(orc, fid, inst, stride, bufs, seed):
     """the 7 witness columns (d1 evaluations) and the 7 sigma columns read at `stride` -> (d_w, d_sigma)"""
-    d_w = [put(ctx, bufs, ev.mont(orc, fid, inst.w[k])) for k in range(7)]
-    d_s = [put(ctx, bufs, pr.sigma_strided(orc, fid, inst.sigma[k], stride, seed + k)) for k in range(7)]
+    d_w = [bufs.put(ev.mont(orc, fid, inst.w[k])) for k in range(7)]
+    d_s = [bufs.put(pr.sigma_strided(orc, fid, inst.sigma[k], stride, seed + k)) for k in range(7)]
     return d_w, d_s
 
 
 def device_z(ctx, orc, fid, log_n, zk_rows, inst, d_w, d_s, stride, bufs):
     n = 1 << log_n
-    d_z = put(ctx, bufs, stale(n))
+    d_z = bufs.put(stale(n))
     ok = ctx.perm_aggreg_dev(fid, log_n, zk_rows, d_w, d_s, stride * n, *scalars(orc, fid, inst), d_z)
     return ctx.dev_download(d_z, (n, 4)), ok, d_z
 
@@ -113,12 +99,9 @@ def test_z_matches_the_reference(ctx, orc, fid, log_n, zk_rows):
         num, den = (num0, den0) if j is None or j >= n - 1 else patch_row(orc, fid, log_n, vi, num0, den0, j)
         z, want_ok = pr.z_evaluations(num, den, zk_rows, vi.rand, P)
         want = ev.mont(orc, fid, pr.interpolate(orc, fid, z))
-        bufs = []
-        try:
-            d_w, d_s = upload(ctx, orc, fid, vi, stride, bufs, seed=log_n + zk_rows)
+        with ctx.buffers() as bufs:
+            d_w, d_s = upload(orc, fid, vi, stride, bufs, seed=log_n + zk_rows)
             got, ok, _ = device_z(ctx, orc, fid, log_n, zk_rows, vi, d_w, d_s, stride, bufs)
-        finally:
-            free_all(ctx, bufs)
         assert ok == want_ok, name
         assert want_ok == (name in ("valid", "zero in the tail", "wired zk row")), name
         assert np.array_equal(got, want), name
@@ -145,19 +128,18 @@ def test_perm_quotient_over_the_device_z_vanishes_on_d1(ctx, orc, fid, log_n, zk
     inst = pr.wired_instance(orc, fid, log_n, zk_rows, seed=77 + fid + log_n + zk_rows)
     beta, gamma, shifts, rand = scalars(orc, fid, inst)
     alpha0 = ev.mont(orc, fid, [random.Random(fid).randrange(1, P)])[0]
-    bufs = []
-    try:
-        d_wev = put(ctx, bufs, np.concatenate([ev.mont(orc, fid, inst.w[k]) for k in range(7)]))
-        d_s8 = put(ctx, bufs, np.concatenate([pr.sigma_d8(orc, fid, inst.sigma[k]) for k in range(7)]))
+    with ctx.buffers() as bufs:
+        d_wev = bufs.put(np.concatenate([ev.mont(orc, fid, inst.w[k]) for k in range(7)]))
+        d_s8 = bufs.put(np.concatenate([pr.sigma_d8(orc, fid, inst.sigma[k]) for k in range(7)]))
         d_w = [d_wev + k * n * 32 for k in range(7)]
         d_s = [d_s8 + k * m8 * 32 for k in range(7)]
-        d_z = put(ctx, bufs, stale(n))
+        d_z = bufs.put(stale(n))
         assert ctx.perm_aggreg_dev(fid, log_n, zk_rows, d_w, d_s, m8, beta, gamma, shifts, rand, d_z) is True
-        d_wc, d_w8, d_z8, d_zk8, d_out = (put(ctx, bufs, np.zeros((k, 4), dtype=np.uint64)) for k in (7 * n, 7 * m8, m8, m8, m8))
+        d_wc, d_w8, d_z8, d_zk8, d_out = (bufs.put(np.zeros((k, 4), dtype=np.uint64)) for k in (7 * n, 7 * m8, m8, m8, m8))
         ctx.ntt_dev_oop(fid, d_wev, n, n, d_wc, log_n, batch=7, inverse=True)             # the witness polynomials
         ctx.ntt_dev_oop(fid, d_wc, n, n, d_w8, log_n + 3, batch=7)                        # ... over d8
         ctx.ntt_dev_oop(fid, d_z, n, n, d_z8, log_n + 3)                                  # z over d8
-        d_zk = put(ctx, bufs, ev.mont(orc, fid, vanishing_coeffs(orc, fid, log_n, zk_rows)))
+        d_zk = bufs.put(ev.mont(orc, fid, vanishing_coeffs(orc, fid, log_n, zk_rows)))
         ctx.ntt_dev_oop(fid, d_zk, 4, 4, d_zk8, log_n + 3)                                # zkpm over d8
         ctx.perm_quotient_dev(fid, log_n + 3, [d_w8 + k * m8 * 32 for k in range(7)], d_z8, d_s, d_zk8, beta, gamma, alpha0, shifts, d_out)
         out = ctx.dev_download(d_out, (m8, 4))
@@ -167,8 +149,6 @@ def test_perm_quotient_over_the_device_z_vanishes_on_d1(ctx, orc, fid, log_n, zk
         at = ctx.poly_evaluate_chunks_dev(fid, [(d_z, n)], 1, n, ev.mont(orc, fid, [1, pow(w, n - zk_rows, P)]))
         one = ev.mont(orc, fid, [1])[0]
         assert np.array_equal(at[0, 0, 0], one) and np.array_equal(at[0, 1, 0], one)
-    finally:
-        free_all(ctx, bufs)
 
 
 # ---------------------------------------------------------------------------------------------------------------- errors, threads
@@ -178,10 +158,9 @@ def test_refusals_leave_z_untouched(ctx, orc):
     inst = pr.wired_instance(orc, fid, log_n, zk_rows, seed=3)
     beta, gamma, shifts, rand = scalars(orc, fid, inst)
     bad = np.array([P & (2**64 - 1), (P >> 64) & (2**64 - 1), (P >> 128) & (2**64 - 1), P >> 192], dtype=np.uint64)
-    bufs = []
-    try:
-        d_w, d_s = upload(ctx, orc, fid, inst, 8, bufs, seed=3)
-        d_z = put(ctx, bufs, stale(n))
+    with ctx.buffers() as bufs:
+        d_w, d_s = upload(orc, fid, inst, 8, bufs, seed=3)
+        d_z = bufs.put(stale(n))
         sh_bad, rn_bad = shifts.copy(), rand.copy()
         sh_bad[6], rn_bad[1] = bad, bad
         cases = [dict(field=7), dict(log_n=31), dict(zk_rows=2), dict(zk_rows=0), dict(zk_rows=n), dict(zk_rows=n + 1),
@@ -221,22 +200,12 @@ def test_refusals_leave_z_untouched(ctx, orc):
         for s in range(1, 9):
             ctx.perm_aggreg_dev(fid, log_n, zk_rows, d_w, d_s, s * n, beta, gamma, shifts, rand, d_z)
         assert ctx.perm_aggreg_dev(fid, log_n, zk_rows, d_w, d_s, 8 * n, beta, gamma, shifts, rand, d_z) is True
-    finally:
-        free_all(ctx, bufs)
 
 
 def test_two_threads_share_a_context(ctx, orc):
     fid, log_n, zk_rows = zk.FP, 12, 6
     P, n = orc.MODULUS[fid], 1 << log_n
-    cases, bufs, errors = [], [], []
-    for t in range(2):
-        inst = pr.wired_instance(orc, fid, log_n, zk_rows, seed=500 + t)
-        if t:
-            k, j = inst.wired[0]
-            inst.w[k][j] = (inst.w[k][j] + 1) % P                     # one thread's instance fails the final-value check
-        _, coeffs, ok = pr.perm_aggreg(orc, fid, log_n, zk_rows, inst.w, inst.sigma, inst.shifts, inst.beta, inst.gamma, inst.rand)
-        d_w, d_s = upload(ctx, orc, fid, inst, 8, bufs, seed=t)
-        cases.append((inst, d_w, d_s, put(ctx, bufs, stale(n)), ev.mont(orc, fid, coeffs), ok))
+    cases, errors = [], []
 
     def work(t):
         try:
@@ -247,13 +216,19 @@ def test_two_threads_share_a_context(ctx, orc):
         except Exception as e:                    # reported by the main thread
             errors.append(e)
 
-    try:
+    with ctx.buffers() as bufs:
+        for t in range(2):
+            inst = pr.wired_instance(orc, fid, log_n, zk_rows, seed=500 + t)
+            if t:
+                k, j = inst.wired[0]
+                inst.w[k][j] = (inst.w[k][j] + 1) % P                     # one thread's instance fails the final-value check
+            _, coeffs, ok = pr.perm_aggreg(orc, fid, log_n, zk_rows, inst.w, inst.sigma, inst.shifts, inst.beta, inst.gamma, inst.rand)
+            d_w, d_s = upload(orc, fid, inst, 8, bufs, seed=t)
+            cases.append((inst, d_w, d_s, bufs.put(stale(n)), ev.mont(orc, fid, coeffs), ok))
         th = [threading.Thread(target=work, args=(t,)) for t in range(2)]
         for t in th:
             t.start()
         for t in th:
             t.join()
-    finally:
-        free_all(ctx, bufs)
     assert not errors, errors
     assert cases[0][5] is True and cases[1][5] is False

@@ -25,15 +25,12 @@ def test_divide_by_vanishing_vs_oracle(ctx, orc, length, log_n):
     fid, n = zk.FQ, 1 << log_n
     f = orc.to_mont(fid, orc.random_scalars(fid, length, seed=length))
     want_q, want_r = orc.divide_by_vanishing(fid, f, log_n)
-    d_f, d_q = ctx.dev_alloc(f.nbytes), ctx.dev_alloc(max(length - n, 1) * 32)
-    try:
-        ctx.dev_upload(d_f, f)
+    with ctx.buffers() as bufs:
+        d_f, d_q = bufs.put(f), bufs.alloc(max(length - n, 1) * 32)
         zero_rem = ctx.poly_divide_by_vanishing_dev(fid, d_f, length, log_n, d_q)
         assert zero_rem == (not want_r.any())
         if length > n:
             assert np.array_equal(ctx.dev_download(d_q, (length - n, 4)), want_q)
-    finally:
-        ctx.dev_free(d_f); ctx.dev_free(d_q)
 
 
 def test_exact_multiple_of_the_vanishing_polynomial_has_zero_remainder(ctx, orc):
@@ -46,16 +43,13 @@ def test_exact_multiple_of_the_vanishing_polynomial_has_zero_remainder(ctx, orc)
         f[j + n] = (f[j + n] + c) % P
         f[j] = (f[j] - c) % P
     fm, qm = orc.to_mont(fid, orc.ints_to_limbs(f)), orc.to_mont(fid, orc.ints_to_limbs(q))
-    d_f, d_q = ctx.dev_alloc(fm.nbytes), ctx.dev_alloc(qm.nbytes)
-    try:
-        ctx.dev_upload(d_f, fm)
+    with ctx.buffers() as bufs:
+        d_f, d_q = bufs.put(fm), bufs.alloc(qm.nbytes)
         assert ctx.poly_divide_by_vanishing_dev(fid, d_f, 8 * n, log_n, d_q) is True
         assert np.array_equal(ctx.dev_download(d_q, (7 * n, 4)), qm)
         fm[3] = orc.to_mont(fid, orc.ints_to_limbs([(f[3] + 1) % P]))[0]                # one coefficient off: remainder != 0
         ctx.dev_upload(d_f, fm)
         assert ctx.poly_divide_by_vanishing_dev(fid, d_f, 8 * n, log_n, d_q) is False
-    finally:
-        ctx.dev_free(d_f); ctx.dev_free(d_q)
 
 
 class QuotientCase:
@@ -134,15 +128,12 @@ class QuotientCase:
 def test_one_quotient_polynomial_without_leaving_the_device(ctx, orc, vesta_srs):
     case = QuotientCase(orc, vesta_srs)
     n, m4, m8 = 1 << case.log_n, 4 << case.log_n, 8 << case.log_n
-    bufs = []
-    bases = ctx.upload_bases(vesta_srs.cid, vesta_srs.g[:n])
-    try:
+    with ctx.upload_bases(vesta_srs.cid, vesta_srs.g[:n]) as bases, ctx.buffers() as bufs:
         d = {}
         for name in QuotientCase.INPUTS:                        # the ONE upload of per-proof data (cols); the rest is per-index, resident
-            a = getattr(case, name)
-            d[name] = ctx.dev_alloc(a.nbytes); bufs.append(d[name]); ctx.dev_upload(d[name], a)
+            d[name] = bufs.put(getattr(case, name))
         for name, nb in case.scratch_bytes().items():
-            d[name] = ctx.dev_alloc(nb); bufs.append(d[name])
+            d[name] = bufs.alloc(nb)
 
         def check(stage):
             if stage == "t":
@@ -152,7 +143,3 @@ def test_one_quotient_polynomial_without_leaving_the_device(ctx, orc, vesta_srs)
         got = case.run_on_device(ctx, d, bases, check)
         for c in range(7):
             assert np.array_equal(got[c], case.want_comm[c]), c
-    finally:
-        bases.free()
-        for p in bufs:
-            ctx.dev_free(p)

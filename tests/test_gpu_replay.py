@@ -16,11 +16,8 @@ sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(
 
 def test_replay_of_a_2_16_proof_every_stage_bit_exact(orc):
     from replay_kimchi import replay
-    ctx = zk.Context(0)
-    try:
+    with zk.Context(0) as ctx:
         rep = replay(zk, orc, ctx, log_n=16, check=True)
-    finally:
-        ctx.close()
     assert rep["checks"]["lagrange_basis_equals_srs_test_vesta"]
     assert all(rep["checks"].values())
     assert set(rep["stages_s"]) <= set(rep["checks"]) | {"lagrange_basis_equals_srs_test_vesta"}

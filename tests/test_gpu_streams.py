@@ -129,21 +129,17 @@ def test_ntt_dev_oop_d1_to_d8(ctx, stream, orc):
 def test_msm_dev(ctx, stream, orc, vesta_srs):
     G, n = vesta_srs, 2048
     sc = orc.random_scalars(G.scalar, n, seed=3)
-    bases = ctx.upload_bases(G.cid, G.g[:n])
-    try:
+    with ctx.upload_bases(G.cid, G.g[:n]) as bases:
         inp = Inputs()
         d = inp(sc)
         r, _ = on_stream(stream, inp, lambda: ctx.msm_dev(bases, d, n))
         assert np.array_equal(zk.jacobian_to_affine(G.cid, r), orc.msm(G.cid, G.g[:n], sc))
-    finally:
-        bases.free()
 
 
 def test_msm_partial_and_finish_gathered(ctx, stream, orc, vesta_srs):
     G, n = vesta_srs, 2048
     sc = orc.random_scalars(G.scalar, n, seed=4)
-    bases = ctx.upload_bases(G.cid, G.g[:n])
-    try:
+    with ctx.upload_bases(G.cid, G.g[:n]) as bases:
         inp = Inputs()
         d = inp(sc)
         d_all = torch.zeros((4096, 16), dtype=torch.int64, device="cuda")
@@ -153,8 +149,6 @@ def test_msm_partial_and_finish_gathered(ctx, stream, orc, vesta_srs):
             return ctx.msm_finish_gathered(G.cid, d_all.data_ptr(), 1, c, g)
         r, _ = on_stream(stream, inp, call)
         assert np.array_equal(zk.jacobian_to_affine(G.cid, r), orc.msm(G.cid, G.g[:n], sc))
-    finally:
-        bases.free()
 
 
 def test_poly_add_and_divide_by_vanishing(ctx, stream, orc):
@@ -328,14 +322,11 @@ def test_one_quotient_polynomial_never_leaving_the_stream(ctx, stream, orc, vest
     d = {name: inp(getattr(case, name)) for name in QuotientCase.INPUTS}
     scratch = {name: stale(nb // 8) for name, nb in case.scratch_bytes().items()}
     d.update({name: t.data_ptr() for name, t in scratch.items()})
-    bases = ctx.upload_bases(vesta_srs.cid, vesta_srs.g[:n])
-    try:
+    with ctx.upload_bases(vesta_srs.cid, vesta_srs.g[:n]) as bases:
         got, (q,) = on_stream(stream, inp, lambda: case.run_on_device(ctx, d, bases), [scratch["q"]])
         assert np.array_equal(q.reshape(-1, 4), case.quot)
         for c in range(7):
             assert np.array_equal(got[c], case.want_comm[c]), c
-    finally:
-        bases.free()
 
 
 # ---------------------------------------------------------------------------------------------------------------- host pointers and handles
@@ -357,15 +348,12 @@ def test_host_pointer_msm_and_msm_batch(ctx, stream, orc, vesta_srs):
     G, n, k = vesta_srs, 2048, 5
     sc = orc.random_scalars(G.scalar, k * n, seed=10).reshape(k, n, 4)
     want = [orc.msm(G.cid, G.g[:n], sc[j]) for j in range(k)]
-    bases = ctx.upload_bases(G.cid, G.g[:n])
-    try:
+    with ctx.upload_bases(G.cid, G.g[:n]) as bases:
         assert np.array_equal(behind_spin(stream, lambda: ctx.msm_affine(bases, sc[0])), want[0])
         assert np.array_equal(behind_spin(stream, lambda: ctx.msm_affine(bases, pinned(sc[1]))), want[1])
         out = behind_spin(stream, lambda: ctx.msm_batch(bases, sc))
         for j in range(k):
             assert np.array_equal(zk.jacobian_to_affine(G.cid, out[j]), want[j]), j
-    finally:
-        bases.free()
 
 
 def check_pinned_ntt_batch(ctx, stream, orc):
@@ -391,16 +379,13 @@ def commit_batch_case(orc, G, n=2048):
 def test_commit_evaluations_batch(ctx, stream, orc, pallas_srs):
     G, n = pallas_srs, 2048
     ev15, lag, want = commit_batch_case(orc, G, n)
-    srs = zk.SRS(ctx, G.cid, G.g[:n], G.mont_points(G.h_xy_canon)[0])
-    try:
+    with zk.SRS(ctx, G.cid, G.g[:n], G.mont_points(G.h_xy_canon)[0]) as srs:
         srs.add_lagrange_basis(n, lag)
         got = behind_spin(stream, lambda: srs.commit_evaluations_non_hiding_batch(n, ev15))
         for j in range(15):
             assert np.array_equal(got[j].chunks[0], want[j]), j
         # the basis built on the device and read back (zk_srs_get_lagrange_basis) on the same stream
         assert np.array_equal(behind_spin(stream, lambda: srs.get_lagrange_basis_from_domain_size(n)), lag)
-    finally:
-        srs.close()
 
 
 def opening_bytes_want():
@@ -420,8 +405,7 @@ def test_srs_open_regression_bytes(ctx, stream, orc, vesta_srs):
 def test_srs_verify(ctx, stream, orc, vesta_srs):
     G, n = vesta_srs, 1024
     g, h = G.g[:n], G.mont_points(G.h_xy_canon)[0]
-    srs = zk.SRS(ctx, G.cid, g, h)
-    try:
+    with zk.SRS(ctx, G.cid, g, h) as srs:
         entries = hash_entries(orc, G, srs, g, h, 2, 31, [n - 3])
         rb, sgb = scales(orc, G, 7)
         ok, pt = behind_spin(stream, lambda: device_verify(orc, G, srs, entries, rb, sgb))
@@ -429,8 +413,6 @@ def test_srs_verify(ctx, stream, orc, vesta_srs):
         bad = tamper(entries, "z1", orc.FP_MODULUS, g[3], at=1)
         ok, pt = behind_spin(stream, lambda: device_verify(orc, G, srs, bad, rb, sgb))
         assert not ok and np.array_equal(pt, oracle_verify(orc, G.cid, g, h, bad, rb, sgb))
-    finally:
-        srs.close()
 
 
 @pytest.mark.parametrize("lanes", [4, 1])
@@ -569,16 +551,13 @@ def test_default_stream_ntt_dev(ctx, orc, on_default_stream):
 def test_default_stream_msm_dev(ctx, orc, pallas_srs, on_default_stream):
     G, n = pallas_srs, 2048
     sc = orc.random_scalars(G.scalar, n, seed=71)
-    bases = ctx.upload_bases(G.cid, G.g[:n])
-    try:
+    with ctx.upload_bases(G.cid, G.g[:n]) as bases:
         warm = dev(sc)
         ctx.msm_dev(bases, warm.data_ptr(), n)           # warm-up, as above
         inp = Inputs()
         d = inp(sc)
         r, _ = on_stream(on_default_stream, inp, lambda: ctx.msm_dev(bases, d, n))
         assert np.array_equal(zk.jacobian_to_affine(G.cid, r), orc.msm(G.cid, G.g[:n], sc))
-    finally:
-        bases.free()
 
 
 # ---------------------------------------------------------------------------------------------------------------- profiled runs
@@ -596,8 +575,7 @@ def test_profiled_msm_batch_and_stage_times(ctx, stream, orc, vesta_srs):
     finite, non-negative stage times"""
     G, n, k = vesta_srs, 2048, 5
     sc = orc.random_scalars(G.scalar, k * n, seed=80).reshape(k, n, 4)
-    bases = ctx.upload_bases(G.cid, G.g[:n])
-    try:
+    with ctx.upload_bases(G.cid, G.g[:n]) as bases:
         plain = [zk.jacobian_to_affine(G.cid, r) for r in ctx.msm_batch(bases, sc)]
         ctx.set_profile(True)
         try:
@@ -615,8 +593,6 @@ def test_profiled_msm_batch_and_stage_times(ctx, stream, orc, vesta_srs):
         times = [st[s] for s in ("recode", "plan", "scatter", "accumulate", "finish", "bitsum")]
         assert all(np.isfinite(t) and t >= 0 for t in times), st
         assert sum(times) > 0, st
-    finally:
-        bases.free()
 
 
 def test_profiled_ntt(ctx, stream, orc, profiled):
@@ -635,14 +611,11 @@ def test_profiled_ntt(ctx, stream, orc, profiled):
 def test_profiled_commit_evaluations_batch(ctx, stream, orc, pallas_srs, profiled):
     G, n = pallas_srs, 2048
     ev15, lag, want = commit_batch_case(orc, G, n)
-    srs = zk.SRS(ctx, G.cid, G.g[:n], G.mont_points(G.h_xy_canon)[0])
-    try:
+    with zk.SRS(ctx, G.cid, G.g[:n], G.mont_points(G.h_xy_canon)[0]) as srs:
         srs.add_lagrange_basis(n, lag)
         got = behind_spin(stream, lambda: srs.commit_evaluations_non_hiding_batch(n, ev15))
         for j in range(15):
             assert np.array_equal(got[j].chunks[0], want[j]), j
-    finally:
-        srs.close()
 
 
 def test_profiled_srs_open_regression_bytes(ctx, stream, orc, vesta_srs, profiled):

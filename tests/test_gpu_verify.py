@@ -114,8 +114,7 @@ def full(request, ctx, orc):
 def test_full_srs_batches_verify(ctx, orc, full, window_bits):
     G, g, h, entries = full
     rb, sgb = scales(orc, G, 3)
-    srs = zk.SRS(ctx, G.cid, g, h, window_bits=window_bits)
-    try:
+    with zk.SRS(ctx, G.cid, g, h, window_bits=window_bits) as srs:
         for B in (1, 16):
             ok, pt = device_verify(orc, G, srs, entries[:B], rb, sgb)
             assert ok and not pt.any(), B
@@ -124,8 +123,6 @@ def test_full_srs_batches_verify(ctx, orc, full, window_bits):
             ok, pt = device_verify(orc, G, srs, bad, rb, sgb)
             assert not ok
             assert np.array_equal(pt, oracle_verify(orc, G.cid, g, h, bad, rb, sgb))
-    finally:
-        srs.close()
 
 
 @pytest.mark.parametrize("n", [48, 128])
@@ -133,8 +130,7 @@ def test_non_power_of_two_srs_chunked_zero_and_empty_commitments(ctx, orc, vesta
     """a 48-point SRS (padded to 64), chunked commitments (polynomials longer than |g|), an identity chunk and an empty PolyComm"""
     G = vesta_srs
     g, h = G.g[:n], G.mont_points(G.h_xy_canon)[0]
-    srs = zk.SRS(ctx, G.cid, g, h)
-    try:
+    with zk.SRS(ctx, G.cid, g, h) as srs:
         entries = hash_entries(orc, G, srs, g, h, 3, n, [n // 2 + 1, 2 * n + 17], zero_poly=True, empty_comm=True)
         assert max(c.shape[0] for c in entries[0].comms) == 3 and entries[0].comms[-1].shape[0] == 0
         rb, sgb = scales(orc, G, 5)
@@ -144,37 +140,31 @@ def test_non_power_of_two_srs_chunked_zero_and_empty_commitments(ctx, orc, vesta
         bad = tamper(entries, "z2", orc.FP_MODULUS, g[3], at=1)
         ok, pt = device_verify(orc, G, srs, bad, rb, sgb)
         assert not ok and np.array_equal(pt, oracle_verify(orc, G.cid, g, h, bad, rb, sgb))
-    finally:
-        srs.close()
 
 
 def test_fewer_rounds_zero_challenge_and_empty_batch(ctx, orc, vesta_srs):
     G = vesta_srs
     g, h = G.g[:128], G.mont_points(G.h_xy_canon)[0]
-    small = zk.SRS(ctx, G.cid, g[:32], h)
-    srs = zk.SRS(ctx, G.cid, g, h)
-    try:
-        short = hash_entries(orc, G, small, g[:32], h, 1, 11, [20])          # 5 rounds: its s covers the first 32 generators
-        full = hash_entries(orc, G, srs, g, h, 2, 12, [100])
-        assert len(short[0].opening.lr) == 5 and len(full[0].opening.lr) == 7
-        rb, sgb = scales(orc, G, 6)
-        batch = [full[0], short[0], full[1]]
-        ok, pt = device_verify(orc, G, srs, batch, rb, sgb)
-        assert ok and not pt.any()
-        assert not oracle_verify(orc, G.cid, g, h, batch, rb, sgb).any()
-        # a transcript that answers 0 in round 2: chal_inv stays 0 (batch_inversion), the proof fails, the sum is the oracle's
-        zero = list(batch)
-        e = zero[0]
-        zero[0] = Entry(e.opening, e.elm, e.polyscale, e.evalscale, e.comms, e.cip,
-                        lambda: HashTranscript(orc.FP_MODULUS, G.g[200:232], 12000, zero_round=2))
-        ok, pt = device_verify(orc, G, srs, zero, rb, sgb)
-        assert not ok and np.array_equal(pt, oracle_verify(orc, G.cid, g, h, zero, rb, sgb))
-        ok, pt = zk.srs_verify(srs, [], mont1(orc, G.scalar, rb), mont1(orc, G.scalar, sgb), return_sum=True)
-        assert ok and not pt.any()
-        assert zk.srs_verify(srs, [], mont1(orc, G.scalar, rb), mont1(orc, G.scalar, sgb)) is True
-    finally:
-        small.close()
-        srs.close()
+    with zk.SRS(ctx, G.cid, g[:32], h) as small:
+        with zk.SRS(ctx, G.cid, g, h) as srs:
+            short = hash_entries(orc, G, small, g[:32], h, 1, 11, [20])          # 5 rounds: its s covers the first 32 generators
+            full = hash_entries(orc, G, srs, g, h, 2, 12, [100])
+            assert len(short[0].opening.lr) == 5 and len(full[0].opening.lr) == 7
+            rb, sgb = scales(orc, G, 6)
+            batch = [full[0], short[0], full[1]]
+            ok, pt = device_verify(orc, G, srs, batch, rb, sgb)
+            assert ok and not pt.any()
+            assert not oracle_verify(orc, G.cid, g, h, batch, rb, sgb).any()
+            # a transcript that answers 0 in round 2: chal_inv stays 0 (batch_inversion), the proof fails, the sum is the oracle's
+            zero = list(batch)
+            e = zero[0]
+            zero[0] = Entry(e.opening, e.elm, e.polyscale, e.evalscale, e.comms, e.cip,
+                            lambda: HashTranscript(orc.FP_MODULUS, G.g[200:232], 12000, zero_round=2))
+            ok, pt = device_verify(orc, G, srs, zero, rb, sgb)
+            assert not ok and np.array_equal(pt, oracle_verify(orc, G.cid, g, h, zero, rb, sgb))
+            ok, pt = zk.srs_verify(srs, [], mont1(orc, G.scalar, rb), mont1(orc, G.scalar, sgb), return_sum=True)
+            assert ok and not pt.any()
+            assert zk.srs_verify(srs, [], mont1(orc, G.scalar, rb), mont1(orc, G.scalar, sgb)) is True
 
 
 class CallbackFailure(Exception):
@@ -184,33 +174,28 @@ class CallbackFailure(Exception):
 def test_errors(ctx, orc, vesta_srs):
     G = vesta_srs
     g, h = G.g[:128], G.mont_points(G.h_xy_canon)[0]
-    srs = zk.SRS(ctx, G.cid, g, h)
-    small = zk.SRS(ctx, G.cid, g[:64], h)
-    try:
-        entries = hash_entries(orc, G, srs, g, h, 2, 21, [50])
-        rb, sgb = (mont1(orc, G.scalar, x) for x in scales(orc, G, 8))
-        with pytest.raises(zk.ZkError) as e:                                   # 7 rounds against a 64-point SRS
-            zk.srs_verify(small, [to_device(zk, orc, G.scalar, x) for x in entries], rb, sgb)
-        assert e.value.code == -4
-        batch = [to_device(zk, orc, G.scalar, x) for x in entries]
+    with zk.SRS(ctx, G.cid, g, h) as srs:
+        with zk.SRS(ctx, G.cid, g[:64], h) as small:
+            entries = hash_entries(orc, G, srs, g, h, 2, 21, [50])
+            rb, sgb = (mont1(orc, G.scalar, x) for x in scales(orc, G, 8))
+            with pytest.raises(zk.ZkError) as e:                                   # 7 rounds against a 64-point SRS
+                zk.srs_verify(small, [to_device(zk, orc, G.scalar, x) for x in entries], rb, sgb)
+            assert e.value.code == -4
+            batch = [to_device(zk, orc, G.scalar, x) for x in entries]
 
-        def boom(j, l, r):
-            raise CallbackFailure("round %d" % j)
-        batch[1].round_challenge = boom
-        with pytest.raises(CallbackFailure):
-            zk.srs_verify(srs, batch, rb, sgb)
-        assert b"round callback failed" in zk.lib().zk_last_error()
-        assert zk.srs_verify(srs, [to_device(zk, orc, G.scalar, x) for x in entries], rb, sgb) is True    # the context still works
-    finally:
-        small.close()
-        srs.close()
+            def boom(j, l, r):
+                raise CallbackFailure("round %d" % j)
+            batch[1].round_challenge = boom
+            with pytest.raises(CallbackFailure):
+                zk.srs_verify(srs, batch, rb, sgb)
+            assert b"round callback failed" in zk.lib().zk_last_error()
+            assert zk.srs_verify(srs, [to_device(zk, orc, G.scalar, x) for x in entries], rb, sgb) is True    # the context still works
 
 
 def test_two_threads_on_one_context(ctx, orc, vesta_srs):
     G = vesta_srs
     g, h = G.g[:128], G.mont_points(G.h_xy_canon)[0]
-    srs = zk.SRS(ctx, G.cid, g, h)
-    try:
+    with zk.SRS(ctx, G.cid, g, h) as srs:
         good = hash_entries(orc, G, srs, g, h, 4, 31, [90])
         bad = tamper(hash_entries(orc, G, srs, g, h, 4, 32, [70]), "sg", orc.FP_MODULUS, g[1], at=0)
         rb, sgb = scales(orc, G, 9)
@@ -231,5 +216,3 @@ def test_two_threads_on_one_context(ctx, orc, vesta_srs):
         assert not errors, errors
         assert all(ok and not pt.any() for ok, pt in results["good"]) and len(results["good"]) == 4
         assert all(not ok and np.array_equal(pt, want_bad) for ok, pt in results["bad"]) and len(results["bad"]) == 4
-    finally:
-        srs.close()

@@ -49,26 +49,17 @@ def run(ctx, zk, orc, torch, log_n, max_poly_size):
     P = orc.FP_MODULUS
     rng = np.random.default_rng(log_n)
     chunks = zk.Context.lagrange_evals_chunks(n, max_poly_size)
-    bufs = []
-
-    def put(a):
-        p = ctx.dev_alloc(a.nbytes)
-        bufs.append(p)
-        ctx.dev_upload(p, a)
-        return p
-
-    try:
-        d_coeffs = put(rand_fe(rng, 17 * n))                                     # w_0..w_14, z, public: coefficients
-        d8 = put(rand_fe(rng, 22 * 8 * n))                                        # s (7) + coefficients8 (15) over d8
+    with ctx.buffers() as bufs:
+        d_coeffs = bufs.put(rand_fe(rng, 17 * n))                                # w_0..w_14, z, public: coefficients
+        d8 = bufs.put(rand_fe(rng, 22 * 8 * n))                                   # s (7) + coefficients8 (15) over d8
         ctx.ntt_dev_oop(fid, d_coeffs, n, n, d8, log_n + 3, batch=1)              # column 0 := w_0 over d8
         one = orc.fe(fid, 1)
-        sel = [put(np.where(rng.integers(0, 2, size=(k * n, 1)) == 1, one, np.uint64(0)).astype(np.uint64)) for k in (4, 4, 8, 8, 8, 8)]
+        sel = [bufs.put(np.where(rng.integers(0, 2, size=(k * n, 1)) == 1, one, np.uint64(0)).astype(np.uint64)) for k in (4, 4, 8, 8, 8, 8)]
         sel_len = [k * n for k in (4, 4, 8, 8, 8, 8)]
         zeta = orc.fe(fid, int(rng.integers(1, 2**62)) * 2**190 + 12345)
         omega = orc.root_of_unity(fid, log_n)
         pts = np.stack([zeta, orc.fe_mul(fid, zeta, omega)])
-        d_bases = [ctx.dev_alloc(chunks * n * 32) for _ in range(2)]
-        bufs += d_bases
+        d_bases = [bufs.alloc(chunks * n * 32) for _ in range(2)]
         columns = [(d8 + k * 8 * n * 32, 8 * n, False) for k in range(22)] + [(p, ln, True) for p, ln in zip(sel, sel_len)]
         polys = [(d_coeffs + j * n * 32, n) for j in range(17)]
         times = {"basis": [], "columns": [], "coeffs": [], "total": []}
@@ -99,9 +90,6 @@ def run(ctx, zk, orc, torch, log_n, max_poly_size):
                 raise SystemExit(f"mismatch: chunk {k} of w_0 at zeta (d1 = 2^{log_n})")
         if not np.array_equal(lag[0], chk[0]):
             raise SystemExit(f"mismatch: Lagrange and coefficient evaluations of w_0 (d1 = 2^{log_n})")
-    finally:
-        for p in bufs:
-            ctx.dev_free(p)
     return {"d1": n, "max_poly_size": max_poly_size, "chunks": chunks, "columns": len(columns), "polys": len(polys), "points": 2,
             **{f"{k}_ms": round(statistics.median(v), 4) for k, v in times.items()}, "check": "ok"}
 
@@ -113,11 +101,8 @@ def main():
     import proof_systems_b200 as zk
     from oracle import oracle as orc
     print(f"card: {card()}")
-    ctx = zk.Context(0)
-    try:
+    with zk.Context(0) as ctx:
         rows = [run(ctx, zk, orc, torch, log_n, m) for log_n, m in CONFIGS]
-    finally:
-        ctx.close()
     print(json.dumps(rows, indent=1))
 
 

@@ -48,18 +48,9 @@ def run(ctx, zk, orc, torch, log_n, m):
     rng = np.random.default_rng(log_n)
     s8, t = rand_fe(rng, 8 * n), rand_fe(rng, 7 * nc * m)
     perm, zeta = rand_fe(rng, 1)[0], rand_fe(rng, 1)[0]
-    bufs = []
-
-    def put(a):
-        p = ctx.dev_alloc(a.nbytes)
-        bufs.append(p)
-        ctx.dev_upload(p, a)
-        return p
-
-    try:
-        d_s8, d_t = put(s8), put(t)
-        d_ft = ctx.dev_alloc(m * 32)
-        bufs.append(d_ft)
+    with ctx.buffers() as bufs:
+        d_s8, d_t = bufs.put(s8), bufs.put(t)
+        d_ft = bufs.alloc(m * 32)
         terms = [(d_s8, 8 * n, perm)]
         times = []
         for rep in range(WARMUP + REPS):
@@ -71,9 +62,6 @@ def run(ctx, zk, orc, torch, log_n, m):
             if rep >= WARMUP:
                 times.append(e0.elapsed_time(e1))
         got = ctx.dev_download(d_ft, (m, 4))
-    finally:
-        for p in bufs:
-            ctx.dev_free(p)
     # the restatement at the timed size
     ints = lambda a: ev.ints(orc, fid, a)
     _, want, want_e1 = fr.ft(orc, fid, log_n, m, [(ints(s8), ints(perm)[0])], ints(t), ints(zeta)[0])
@@ -93,11 +81,8 @@ def main():
     from oracle import oracle as orc
     orc.lib()
     print(f"card: {card()}")
-    ctx = zk.Context(0)
-    try:
+    with zk.Context(0) as ctx:
         rows = [run(ctx, zk, orc, torch, log_n, m) for log_n, m in CONFIGS]
-    finally:
-        ctx.close()
     print(json.dumps(rows, indent=1))
 
 

@@ -62,24 +62,15 @@ def run(ctx, zk, orc, torch, log_n, zk_rows):
     cols8 = [orc.to_mont(fid, orc.random_scalars(fid, 8 * n, seed=k)) for k in range(4)]
     t8 = orc.to_mont(fid, orc.random_scalars(fid, 8 * n, seed=9))
     t8[::8] = mont(inst.T1)
-    bufs = []
-
-    def put(a):
-        a = np.ascontiguousarray(a, dtype=np.uint64)
-        p = ctx.dev_alloc(a.nbytes)
-        bufs.append(p)
-        ctx.dev_upload(p, a)
-        return p
-
     row = {"d1": n, "zk_rows": zk_rows, "m": M}
-    try:
-        d_c = [put(c) for c in cols8[:3]]
-        d_ids = put(cols8[3])
-        d_o8, d_o1 = put(np.zeros((8 * n, 4))), put(np.zeros((n, 4)))
-        d_w = [put(mont(c)) for c in inst.w]
-        d_t = put(t8)
-        d_s = [put(np.zeros((n, 4))) for _ in range(M + 1)]
-        d_a = put(np.zeros((n, 4)))
+    with ctx.buffers() as bufs:
+        d_c = [bufs.put(c) for c in cols8[:3]]
+        d_ids = bufs.put(cols8[3])
+        d_o8, d_o1 = bufs.put(np.zeros((8 * n, 4))), bufs.put(np.zeros((n, 4)))
+        d_w = [bufs.put(mont(c)) for c in inst.w]
+        d_t = bufs.put(t8)
+        d_s = [bufs.put(np.zeros((n, 4))) for _ in range(M + 1)]
+        d_a = bufs.put(np.zeros((n, 4)))
         jc, tic = mont([inst.jc, inst.tic])
         b, g = mont([inst.beta, inst.gamma])
         rs, ra = mont(inst.rand_sorted), mont(inst.rand_agg)
@@ -89,9 +80,6 @@ def run(ctx, zk, orc, torch, log_n, zk_rows):
         got8, got1 = ctx.dev_download(d_o8, (8 * n, 4)), ctx.dev_download(d_o1, (n, 4))
         got_s = [ctx.dev_download(p, (n, 4)) for p in d_s]
         got_a = ctx.dev_download(d_a, (n, 4))
-    finally:
-        for p in bufs:
-            ctx.dev_free(p)
     # the restatement at the timed size
     ints = lambda a: ev.ints(orc, fid, a)
     sub = slice(None) if log_n <= 17 else slice(None, None, 8)
@@ -116,12 +104,9 @@ def main():
     from oracle import oracle as orc
     orc.lib()
     print(f"card: {card()}")
-    ctx = zk.Context(0)
-    ctx.set_stream(torch.cuda.current_stream().cuda_stream)      # the events' stream: the joint table returns with work queued
-    try:
+    with zk.Context(0) as ctx:
+        ctx.set_stream(torch.cuda.current_stream().cuda_stream)      # the events' stream: the joint table returns with work queued
         rows = [run(ctx, zk, orc, torch, log_n, zk_rows) for log_n, zk_rows in CONFIGS]
-    finally:
-        ctx.close()
     print(json.dumps(rows, indent=1))
 
 

@@ -47,20 +47,10 @@ def run(ctx, zk, orc, torch, log_n, zk_rows):
     rng = np.random.default_rng(log_n)
     w, s8 = rand_fe(rng, 7 * n).reshape(7, n, 4), rand_fe(rng, 7 * 8 * n).reshape(7, 8 * n, 4)
     beta, gamma, shifts, rand = rand_fe(rng, 1)[0], rand_fe(rng, 1)[0], rand_fe(rng, 7), rand_fe(rng, 2)
-    bufs = []
-
-    def put(a):
-        a = np.ascontiguousarray(a)
-        p = ctx.dev_alloc(a.nbytes)
-        bufs.append(p)
-        ctx.dev_upload(p, a)
-        return p
-
-    try:
-        d_w = [put(w[k]) for k in range(7)]
-        d_s = [put(s8[k]) for k in range(7)]
-        d_z = ctx.dev_alloc(n * 32)
-        bufs.append(d_z)
+    with ctx.buffers() as bufs:
+        d_w = [bufs.put(w[k]) for k in range(7)]
+        d_s = [bufs.put(s8[k]) for k in range(7)]
+        d_z = bufs.alloc(n * 32)
         times = []
         for rep in range(WARMUP + REPS):
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -74,9 +64,6 @@ def run(ctx, zk, orc, torch, log_n, zk_rows):
         ctx.perm_aggreg_dev(fid, log_n, zk_rows, d_w, d_s, 8 * n, beta, gamma, shifts, rand, d_z)
         launches = ctx.launch_count - launches0
         got = ctx.dev_download(d_z, (n, 4))
-    finally:
-        for p in bufs:
-            ctx.dev_free(p)
     # the restatement at the timed size
     ints = lambda a: ev.ints(orc, fid, a)
     _, want, want_ok = pr.perm_aggreg(orc, fid, log_n, zk_rows, [ints(w[k]) for k in range(7)], [ints(s8[k][::8]) for k in range(7)],
@@ -95,11 +82,8 @@ def main():
     from oracle import oracle as orc
     orc.lib()
     print(f"card: {card()}")
-    ctx = zk.Context(0)
-    try:
+    with zk.Context(0) as ctx:
         rows = [run(ctx, zk, orc, torch, log_n, zk_rows) for log_n, zk_rows in CONFIGS]
-    finally:
-        ctx.close()
     print(json.dumps(rows, indent=1))
 
 

@@ -132,8 +132,6 @@ def replay(zk, orc, ctx, log_n=LOG_N, check=True, n_open_polys=45):
     #      iFFT(n) -> FFT(8n) (out of place into the d8 buffers the quotient reads) -> iFFT(4n) + iFFT(8n), nothing leaves the device.
     #      Results are compared with what the host-path stages above produced (themselves checked against the oracle below).
     cols16 = np.concatenate([wit_m, dense[0:1]])
-    d_cols, d_ev8 = ctx.dev_alloc(cols16.nbytes), ctx.dev_alloc(16 * 8 * N * 32)
-    d_big, d_big4 = ctx.dev_alloc(8 * N * 32), ctx.dev_alloc(4 * N * 32)
     res_r = {}
 
     def rstage(name, fn):
@@ -143,7 +141,9 @@ def replay(zk, orc, ctx, log_n=LOG_N, check=True, n_open_polys=45):
         fn()
         sync()
         res_r[name] = time.perf_counter() - t0
-    try:
+    with ctx.buffers() as bufs:
+        d_cols, d_ev8 = bufs.alloc(cols16.nbytes), bufs.alloc(16 * 8 * N * 32)
+        d_big, d_big4 = bufs.alloc(8 * N * 32), bufs.alloc(4 * N * 32)
         for rep in range(2):                                  # the second pass is the measurement (tables and buffers warm)
             rstage("upload of the 16 evaluation columns (32 B x 16 n)", lambda: ctx.dev_upload(d_cols, cols16))
             ctx.dev_upload(d_big, big); ctx.dev_upload(d_big4, big[: 4 * N])
@@ -154,9 +154,6 @@ def replay(zk, orc, ctx, log_n=LOG_N, check=True, n_open_polys=45):
         assert np.array_equal(got[:15], p_wit2) and np.array_equal(got[15], p_dense[0]), "resident iFFT(n) differs from the host path"
         assert np.array_equal(ctx.dev_download(d_ev8, (16, 8 * N, 4)), p_pad), "resident FFT(8n) differs from the host path"
         assert np.array_equal(ctx.dev_download(d_big, (8 * N, 4)), p_big) and np.array_equal(ctx.dev_download(d_big4, (4 * N, 4)), p_big4)
-    finally:
-        for ptr in (d_cols, d_ev8, d_big, d_big4):
-            ctx.dev_free(ptr)
     report["resident_stages_s"] = res_r
     if not check:
         srs.close()
