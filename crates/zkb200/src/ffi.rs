@@ -176,6 +176,8 @@ extern "C" {
 
     pub fn zk_srs_create(ctx: *mut zk_ctx, curve_id: c_int, g_xy: *const u64, n: usize, h_xy: *const u64, window_bits: c_int,
                          out: *mut *mut zk_srs) -> c_int;
+    pub fn zk_srs_generate(ctx: *mut zk_ctx, curve_id: c_int, depth: usize, window_bits: c_int, g_xy_out: *mut u64, h_xy_out: *mut u64,
+                           out: *mut *mut zk_srs) -> c_int;
     pub fn zk_srs_destroy(srs: *mut zk_srs);
     pub fn zk_srs_lagrange_basis(srs: *mut zk_srs, domain_size: usize, window_bits: c_int) -> c_int;
     pub fn zk_srs_lagrange_basis_chunks(srs: *const zk_srs, domain_size: usize) -> usize;

@@ -86,7 +86,7 @@ impl Drop for SrsHandle {
 /// `ipa::SRS<G>` plus its resident copy on the device.
 #[derive(Clone)]
 pub struct GpuSRS<G: GpuCurve> {
-    /// g, h and everything that never touches an MSM (serde, `create`, verification) stay with the reference type
+    /// g, h and everything that never touches an MSM (serde, verification) stay with the reference type
     pub inner: Arc<ipa::SRS<G>>,
     pub(crate) ctx: Arc<Ctx>,
     pub(crate) dev: Arc<SrsHandle>,
@@ -217,9 +217,16 @@ impl<G: GpuCurve> SRS<G> for GpuSRS<G> {
         self.mask_custom(self.commit_evaluations_non_hiding(domain, plnm), blinders)
     }
 
-    /// ipa.rs:751-778: the generators come from the reference's own hash-to-curve; only their resident copy is new
+    /// ipa.rs:751-778 — `zk_srs_generate`: g and h are hashed to the curve on the device and stay resident in the handle that call
+    /// returns; `inner` is built from the host copies, so nothing is uploaded again
     fn create(depth: usize) -> Self {
-        Self::from_srs(<ipa::SRS<G> as SRS<G>>::create(depth), Ctx::global()).expect("zkb200: SRS upload")
+        let ctx = Ctx::global();
+        let mut g = vec![0u64; 8 * depth];
+        let mut h = [0u64; 8];
+        let mut dev = core::ptr::null_mut();
+        check(unsafe { zk_srs_generate(ctx.0, G::CURVE_ID, depth, -1, g.as_mut_ptr(), h.as_mut_ptr(), &mut dev) }).expect("zkb200: SRS::create");
+        let inner = ipa::SRS::new(g.chunks_exact(8).map(G::from_limbs).collect(), G::from_limbs(&h));
+        Self { inner: Arc::new(inner), ctx, dev: Arc::new(SrsHandle(dev)), lagrange: Arc::new(Mutex::new(HashMap::new())) }
     }
 
     fn get_lagrange_basis(&self, domain: D<G::ScalarField>) -> impl Deref<Target = Vec<PolyComm<G>>> + '_ {

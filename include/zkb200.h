@@ -189,6 +189,12 @@ int zk_dev_download(zk_ctx* ctx, void* dst, const void* d_src, size_t bytes);
  *                          CommitmentError::BlindersDontMatch (poly-commitment/src/error.rs:3-9) */
 int zk_srs_create(zk_ctx* ctx, int curve_id, const uint64_t* g_xy, size_t n, const uint64_t h_xy[8], int window_bits,
                   zk_srs** out);
+/* SRS::create(depth) (ipa.rs:751-778), generated on the device: g[i] = point_of_random_bytes(Blake2b512(u32_be(i))) for
+ * i < depth and h = point_of_random_bytes(Blake2b512(b"srs_misc" || u32_be(0))), the Blake2b digest mapped to the curve by the
+ * BW group map (ipa.rs:234-265, groupmap/src/lib.rs).  Any depth in [1, 2^32]; the points never pass through the host.
+ * g_xy_out (depth x 8 u64) and h_xy_out: optional affine Montgomery copies for the host, NULL to skip.  window_bits as in
+ * zk_bases_upload.  ZK_ERR_INVALID, before any allocation, for a bad curve, a NULL out, depth 0 or depth > 2^32. */
+int zk_srs_generate(zk_ctx* ctx, int curve_id, size_t depth, int window_bits, uint64_t* g_xy_out, uint64_t h_xy_out[8], zk_srs** out);
 void zk_srs_destroy(zk_srs* srs);
 size_t zk_srs_max_poly_size(const zk_srs* srs);
 int zk_srs_add_lagrange_basis(zk_srs* srs, size_t domain_size, const uint64_t* basis_xy, int window_bits);

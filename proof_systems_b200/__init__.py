@@ -5,6 +5,7 @@ csrc/).  This package is the thin Python host layer used by the tests and bench.
 reference's interfaces on this path, with the reference's names:
 
     SRS.commit_non_hiding / commit_evaluations_non_hiding / mask_custom    poly-commitment/src/ipa.rs:605-728
+    SRS.create                                                             poly-commitment/src/ipa.rs:751-778
     PolyComm                                                               poly-commitment/src/commitment.rs:47-50
     Radix2EvaluationDomain.fft_in_place / ifft_in_place                    ark_poly (kimchi/src/circuits/domains.rs:24-33)
     LagrangeBasisEvaluations.new / evaluate / evaluate_boolean             kimchi/src/lagrange_basis_evaluations.rs:72-258

@@ -140,6 +140,7 @@ def lib() -> ctypes.CDLL:
                                        ctypes.POINTER(ctypes.c_int64)]
     L.zk_lookup_aggreg_dev.argtypes = [vp, i, u, sz, ctypes.POINTER(vp), vp, u, ctypes.POINTER(LookupInfo), ctypes.POINTER(vp), vp, vp, vp, vp,
                                        ctypes.POINTER(i)]
+    L.zk_srs_generate.argtypes = [vp, i, sz, i, _u64p, _u64p, ctypes.POINTER(vp)]
     return L
 
 

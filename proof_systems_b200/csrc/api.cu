@@ -457,7 +457,7 @@ int zk_ctx_last_stage_ms(const zk_ctx* ctx, float* out, size_t capacity) {
 int zk_bases_upload(zk_ctx* ctx, int curve_id, const uint64_t* xy_mont, size_t n, int window_bits, int points_on_device, zk_bases** out) {
     if (!ctx || !out || (!xy_mont && n)) { zk_set_error("bases_upload: null argument"); return ZK_ERR_INVALID; }
     if (int rc = check_curve("bases_upload", curve_id)) return rc;
-    if (window_bits < -1 || window_bits == 1 || window_bits > (int)MSM_MAX_WINDOW_BITS) { zk_set_error("bases_upload: window_bits %d not in {-1, 0, 2..%u}", window_bits, MSM_MAX_WINDOW_BITS); return ZK_ERR_INVALID; }
+    if (int rc = check_table_window("bases_upload", window_bits)) return rc;
     std::lock_guard<std::mutex> lk(ctx->mu);
     ZK_CUDA(cudaSetDevice(ctx->device));
     unsigned c = window_bits < 0 ? (unsigned)msm_default_window(n, true) : (unsigned)window_bits;

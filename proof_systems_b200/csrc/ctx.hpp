@@ -40,6 +40,14 @@ inline int check_curve(const char* what, int curve_id) {
     what ? zk_set_error("%s: unknown curve_id %d", what, curve_id) : zk_set_error("unknown curve_id %d", curve_id);
     return ZK_ERR_INVALID;
 }
+// the window of a resident table: -1 (the default for the size), 0 (no table) or 2..MSM_MAX_WINDOW_BITS
+inline int check_table_window(const char* what, int window_bits) {
+    if (window_bits < -1 || window_bits == 1 || window_bits > (int)MSM_MAX_WINDOW_BITS) {
+        zk_set_error("%s: window_bits %d not in {-1, 0, 2..%u}", what, window_bits, MSM_MAX_WINDOW_BITS);
+        return ZK_ERR_INVALID;
+    }
+    return ZK_OK;
+}
 // domains of up to 2^30 points, the NTT's limit
 inline int check_log_n(const char* what, unsigned log_n, const char* name = "log_n") {
     if (log_n > 30) { zk_set_error("%s: %s %u > 30", what, name, log_n); return ZK_ERR_INVALID; }

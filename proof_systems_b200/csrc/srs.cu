@@ -17,6 +17,10 @@
 
 using namespace zkb;
 
+namespace zkb {
+template <class F> int srs_generate_points(affine_t* d_out, size_t depth, int sm_count, cudaStream_t st);   // srs_gen.cu
+}
+
 // SRS::mask_custom (ipa.rs:605-622): chunk_i + blinder_i * h; one scalar multiplication per chunk, host side.
 template <class HP, class HS> static void mask_one(const uint64_t* chunk, const uint64_t* blinder_mont, const uint64_t* h, uint64_t* out) {
     using namespace host;
@@ -43,6 +47,41 @@ int zk_srs_create(zk_ctx* ctx, int curve_id, const uint64_t* g_xy, size_t n, con
     zk_srs* s = new zk_srs();
     s->ctx = ctx; s->curve = curve_id; s->n = n; s->g = g;
     memcpy(s->h, h_xy, 64);
+    *out = s;
+    return ZK_OK;
+}
+
+// SRS::create(depth) (ipa.rs:751-778): the generators and h hashed to the curve on the device (srs_gen.cu), then made resident
+// like a device-built Lagrange basis.  The lock is held while generating, not across zk_bases_upload, which takes it itself; the
+// upload's synchronisation is the call's only one, and it also completes the copies to the optional host outputs.
+int zk_srs_generate(zk_ctx* ctx, int curve_id, size_t depth, int window_bits, uint64_t* g_xy_out, uint64_t h_xy_out[8], zk_srs** out) {
+    if (!ctx || !out) { zk_set_error("srs_generate: null argument"); return ZK_ERR_INVALID; }
+    if (int rc = check_curve("srs_generate", curve_id)) return rc;
+    // the reference hashes `i as u32`: past 2^32 points the generators would repeat
+    if (depth == 0 || depth > ((size_t)1 << 32)) { zk_set_error("srs_generate: depth %zu not in [1, 2^32]", depth); return ZK_ERR_INVALID; }
+    if (int rc = check_table_window("srs_generate", window_bits)) return rc;
+    DevScratch d_pts;                    // g[0..depth) then h; transient: freed on every return
+    uint64_t h[8];
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        ZK_CUDA(cudaSetDevice(ctx->device));
+        if (int rc = d_pts.ensure((depth + 1) * sizeof(affine_t))) return rc;
+        int rc = with_curve(curve_id, [&](auto cv) { return srs_generate_points<typename decltype(cv)::F>(d_pts.at<affine_t>(), depth, ctx->sm_count, ctx->stream); });
+        if (rc) return rc;
+        ctx->launches += 1;
+        ZK_CUDA(cudaMemcpyAsync(h, d_pts.at<affine_t>() + depth, sizeof(affine_t), cudaMemcpyDeviceToHost, ctx->stream));
+        if (g_xy_out) ZK_CUDA(cudaMemcpyAsync(g_xy_out, d_pts.p, depth * sizeof(affine_t), cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    zk_bases* g = nullptr;
+    int rc = zk_bases_upload(ctx, curve_id, d_pts.at<const uint64_t>(), depth, window_bits, /*points_on_device=*/1, &g);
+    if (rc) {
+        cudaStreamSynchronize(ctx->stream);   // the host copies may still be in flight
+        return rc;
+    }
+    zk_srs* s = new zk_srs();
+    s->ctx = ctx; s->curve = curve_id; s->n = depth; s->g = g;
+    memcpy(s->h, h, sizeof h);
+    if (h_xy_out) memcpy(h_xy_out, h, sizeof h);
     *out = s;
     return ZK_OK;
 }

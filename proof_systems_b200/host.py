@@ -33,12 +33,24 @@ class PolyComm:
 class SRS(Handle):
     """ipa::SRS<G>{g, h, lagrange_bases} with g (and every registered Lagrange basis) resident on the device."""
 
-    def __init__(self, ctx: Context, curve: int, g, h, window_bits: int = -1):
+    def __init__(self, ctx: Context, curve: int, g, h, window_bits: int = -1, _create=None):
+        """_create(g, h, out): the library call that writes the handle, and g and h with it (SRS.create); by default zk_srs_create
+        of g and h"""
         self.ctx, self.curve = ctx, curve
         self.g = _np_u64(g, (8,))
         self.h = _fe(h, 8)
+        if _create is None:
+            _create = lambda g, h, out: lib().zk_srs_create(ctx._h, curve, _ptr(g), g.shape[0], h.ctypes.data_as(_u64p), window_bits, out)
         self._h = ctypes.c_void_p()
-        check(lib().zk_srs_create(ctx._h, curve, _ptr(self.g), self.g.shape[0], self.h.ctypes.data_as(_u64p), window_bits, ctypes.byref(self._h)))
+        check(_create(self.g, self.h, ctypes.byref(self._h)))
+
+    # fn create(depth: usize) -> Self
+    @classmethod
+    def create(cls, ctx: Context, curve: int, depth: int, window_bits: int = -1) -> "SRS":
+        """SRS::create (ipa.rs:751-778): g[0..depth) and h hashed to the curve on the device (zk_srs_generate), bit-exact with the
+        reference; `g` and `h` are the host copies of the points the handle holds."""
+        return cls(ctx, curve, np.empty((depth, 8), dtype=np.uint64), np.empty(8, dtype=np.uint64), _create=lambda g, h, out: lib().zk_srs_generate(
+            ctx._h, curve, depth, window_bits, g.ctypes.data_as(_u64p), h.ctypes.data_as(_u64p), out))
 
     @classmethod
     def from_file(cls, ctx: Context, curve: int, path: str, window_bits: int = -1, lagrange: bool = True) -> "SRS":
