@@ -169,6 +169,31 @@ pub struct zk_lin_term {
     pub coeff: [u64; 4],
 }
 
+/// zk_lookup_table: one LookupTable, its `width` columns of `len` Montgomery elements back to back (column-major)
+#[repr(C)]
+#[derive(Copy, Clone)]
+pub struct zk_lookup_table {
+    pub id: i32,
+    pub width: u32,
+    pub len: u64,
+    pub data: *const u64,
+}
+
+/// zk_runtime_table_cfg: one RuntimeTableCfg, its first column of `len` Montgomery elements
+#[repr(C)]
+#[derive(Copy, Clone)]
+pub struct zk_runtime_table_cfg {
+    pub id: i32,
+    pub len: u64,
+    pub first_column: *const u64,
+}
+
+/// the LookupError kinds zk_lookup_index_build reports (kimchi/src/circuits/lookup/index.rs:23-36)
+pub const ZK_LOOKUP_ERR_NONE: c_int = 0;
+pub const ZK_LOOKUP_ERR_ID_COLLISION: c_int = 1;
+pub const ZK_LOOKUP_ERR_TABLE_ID_ZERO: c_int = 2;
+pub const ZK_LOOKUP_ERR_TOO_LONG: c_int = 3;
+
 extern "C" {
     pub fn zk_last_error() -> *const c_char;
     pub fn zk_ctx_create(device_id: c_int, out: *mut *mut zk_ctx) -> c_int;
@@ -245,4 +270,10 @@ extern "C" {
                           gate_coeffs: *const c_void, gate_coeffs_len: usize, zero_selectors: c_int, out: *mut *mut zk_index_cache) -> c_int;
     pub fn zk_index_commitments(srs: *mut zk_srs, index: *const zk_index_cache, out_xy: *mut u64, capacity_points: usize,
                                 out_points: *mut usize) -> c_int;
+    pub fn zk_lookup_index_build(ctx: *mut zk_ctx, field_id: c_int, domain_d1_size: u64, zk_rows: u64, gates: *const c_void, n_gates: usize,
+                                 tables: *const zk_lookup_table, n_tables: usize, runtime: *const zk_runtime_table_cfg, n_runtime: usize,
+                                 has_runtime: c_int, lookup_error: *mut c_int, runtime_table_offset: *mut u64,
+                                 out: *mut *mut zk_index_cache) -> c_int;
+    pub fn zk_lookup_index_commitments(srs: *mut zk_srs, lookup_index: *const zk_index_cache, out_xy: *mut u64, capacity_points: usize,
+                                       out_points: *mut usize) -> c_int;
 }

@@ -17,7 +17,8 @@
 //!   from the resident witness and `permutation_coefficients8`, leaving z resident (`zk_perm_aggreg_dev`).
 //! * [`index::DeviceIndex`] builds the prover index's column evaluations (kimchi/src/circuits/constraints.rs:510-760) on the device
 //!   from `cs.gates` and the commitments of its verifier index (kimchi/src/verifier_index.rs:221-300) (`zk_index_build`,
-//!   `zk_index_commitments`).
+//!   `zk_index_commitments`); [`index::DeviceLookupIndex`] does the same for the lookup index (kimchi/src/circuits/lookup/index.rs:
+//!   202-482) and the lookup commitments of the verifier index (`zk_lookup_index_build`, `zk_lookup_index_commitments`).
 //! * [`lookup::LookupLowering`] builds the lookup argument's joint table, sorted columns and aggregation polynomial
 //!   (kimchi/src/prover.rs:383-673) from the resident witness and the index cache's lookup tables (`zk_lookup_*_dev`).
 //!

@@ -555,6 +555,44 @@ int zk_index_build(zk_ctx* ctx, int field_id, const zk_index_header* hdr, const 
                    size_t gate_coeffs_len, int zero_selectors, zk_index_cache** out);
 int zk_index_commitments(zk_srs* srs, const zk_index_cache* index, uint64_t* out_xy, size_t capacity_points, size_t* out_points);
 
+/* ------------------------------------------------------------------ lookup index built on the device
+ * zk_lookup_index_build        LookupConstraintSystem::create (kimchi/src/circuits/lookup/index.rs:202-482) from the circuit's gates
+ *                              (PrunedGate records as for zk_index_build, rows n_gates .. n - 1 Zero gates), the fixed lookup tables
+ *                              (LookupTable::data: width x len Montgomery elements, column-major) and, with has_runtime, the runtime
+ *                              table configs (RuntimeTableCfg; has_runtime with n_runtime = 0 is Some(vec![])), into a handle that
+ *                              zk_index_cache_section / _header / _free serve.  Patterns per LookupPattern::from_gate (Lookup; RangeCheck0,
+ *                              RangeCheck1 on rows i and i + 1, Rot64; ForeignFieldMul on rows i and i + 1; Xor16).  The table is the fixed
+ *                              tables as given, then the range-check table (id 1, 0 .. 4095) if RangeCheck or ForeignFieldMul is used and
+ *                              the XOR table (id 0, reversed rows) if Xor is, then one [first_column, 0] table per runtime config;
+ *                              w = max(widest table, max_joint_size) columns, zero past the tables.  Sections, Montgomery, over d8:
+ *                              0x50 the w table columns back to back (elem_domain_size = w), 0x51 table_ids8 (if some table id is
+ *                              nonzero), 0x52 .. 0x55 the selectors of the present patterns xor, lookup, range_check, ffmul, 0x56 the
+ *                              runtime selector (with has_runtime: 1 except on the runtime rows and the last zk_rows rows).  The header
+ *                              holds domain_d1_size, zk_rows and lookup_selectors_present (bit 0 table ids, bits 1 .. 4 the selectors,
+ *                              bit 5 the runtime selector).  *runtime_table_offset (the fixed and gate tables' rows) is written when
+ *                              has_runtime and a handle is made.  No pattern: ZK_OK with *out = NULL.  A LookupError: ZK_ERR_INVALID,
+ *                              *out = NULL, *lookup_error its kind (checked in the reference's order: an id collision between the fixed
+ *                              and the gate tables, then among the runtime tables; id 0 without an all-zero row; len >= n - zk_rows - 1)
+ *                              and zk_last_error the reference's message.  ZK_ERR_INVALID with *lookup_error = 0 for a null pointer, an
+ *                              unknown field, n not a power of two up to 2^27, zk_rows outside [1, n - 2], n_gates > n, a tag > 13, a
+ *                              table width outside 1 .. 16, an entry that is not a canonical field element, runtime tables without
+ *                              has_runtime, a Next pattern on the last row or more table rows than n with runtime tables (the reference
+ *                              panics).  Every check runs on the host before any device work; the call synchronises once.
+ * zk_lookup_index_commitments  the commitments of LookupVerifierIndex (kimchi/src/verifier_index.rs:196-215) for any handle with
+ *                              section 0x50: lookup_table[0 .. w) and table_ids masked with blinder one (every chunk + h), then the
+ *                              selectors xor, lookup, range_check, ffmul and runtime_tables_selector present per the header's bits,
+ *                              not masked; zk_srs_lagrange_basis_chunks(srs, n) points each, commitment-major.  The d1 Lagrange basis is
+ *                              built if the SRS has none.  ZK_ERR_INVALID: a null pointer, a built index of another field than the
+ *                              SRS's scalar field, 0x50 or a section of a header bit missing or of the wrong length, capacity too small. */
+typedef struct zk_lookup_table { int32_t id; uint32_t width; uint64_t len; const uint64_t* data; } zk_lookup_table;
+typedef struct zk_runtime_table_cfg { int32_t id; uint64_t len; const uint64_t* first_column; } zk_runtime_table_cfg;
+enum { ZK_LOOKUP_ERR_NONE = 0, ZK_LOOKUP_ERR_ID_COLLISION = 1, ZK_LOOKUP_ERR_TABLE_ID_ZERO = 2, ZK_LOOKUP_ERR_TOO_LONG = 3 };
+int zk_lookup_index_build(zk_ctx* ctx, int field_id, uint64_t domain_d1_size, uint64_t zk_rows, const void* gates, size_t n_gates,
+                          const zk_lookup_table* tables, size_t n_tables, const zk_runtime_table_cfg* runtime, size_t n_runtime,
+                          int has_runtime, int* lookup_error, uint64_t* runtime_table_offset, zk_index_cache** out);
+int zk_lookup_index_commitments(zk_srs* srs, const zk_index_cache* lookup_index, uint64_t* out_xy, size_t capacity_points,
+                                size_t* out_points);
+
 /* ------------------------------------------------------------------ diagnostics (tests/test_gpu_field.py, DESIGN.md compute model)
  * Element-wise device field ops on n elements (op: 0 mul, 1 add, 2 sub, 3 inverse of a), host pointers. */
 int zk_debug_field_op(zk_ctx* ctx, int field_id, int op, const uint64_t* a, const uint64_t* b, uint64_t* out, size_t n);

@@ -141,6 +141,9 @@ def lib() -> ctypes.CDLL:
     L.zk_lookup_aggreg_dev.argtypes = [vp, i, u, sz, ctypes.POINTER(vp), vp, u, ctypes.POINTER(LookupInfo), ctypes.POINTER(vp), vp, vp, vp, vp,
                                        ctypes.POINTER(i)]
     L.zk_srs_generate.argtypes = [vp, i, sz, i, _u64p, _u64p, ctypes.POINTER(vp)]
+    L.zk_lookup_index_build.argtypes = [vp, i, ctypes.c_uint64, ctypes.c_uint64, vp, sz, ctypes.POINTER(LookupTable), sz,
+                                        ctypes.POINTER(RuntimeTableCfg), sz, i, ctypes.POINTER(i), ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(vp)]
+    L.zk_lookup_index_commitments.argtypes = [vp, vp, _u64p, sz, ctypes.POINTER(sz)]
     return L
 
 
@@ -195,6 +198,16 @@ class LookupInfo(ctypes.Structure):
                 ("n_lookups", ctypes.c_size_t), ("pattern_first", ctypes.POINTER(ctypes.c_uint32)), ("pattern_count", ctypes.POINTER(ctypes.c_uint32)),
                 ("n_patterns", ctypes.c_size_t), ("row_pattern", ctypes.POINTER(ctypes.c_uint8)), ("max_per_row", ctypes.c_uint),
                 ("joint_combiner", ctypes.c_uint64 * 4), ("table_id_combiner", ctypes.c_uint64 * 4), ("dummy", ctypes.c_uint64 * 4)]
+
+
+class LookupTable(ctypes.Structure):
+    """zk_lookup_table (include/zkb200.h)"""
+    _fields_ = [("id", ctypes.c_int32), ("width", ctypes.c_uint32), ("len", ctypes.c_uint64), ("data", ctypes.c_void_p)]
+
+
+class RuntimeTableCfg(ctypes.Structure):
+    """zk_runtime_table_cfg (include/zkb200.h)"""
+    _fields_ = [("id", ctypes.c_int32), ("len", ctypes.c_uint64), ("first_column", ctypes.c_void_p)]
 
 
 class OpenPoly(ctypes.Structure):

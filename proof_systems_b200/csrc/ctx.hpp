@@ -169,6 +169,14 @@ int ctx_msm_many(zk_ctx* ctx, const zk_bases* bases, size_t off, size_t n, const
 // the same with one base offset per MSM (the chunks of a chunked Lagrange basis share their scalars, not their bases)
 int ctx_msm_many_offs(zk_ctx* ctx, const zk_bases* bases, const size_t* offs, size_t n, const fe* const* d_scalars, size_t k, int mont, int window_bits,
                       uint64_t* out_xyz, const affine_t* d_extra = nullptr, size_t n_extra = 0);
+// ctx_ntt_device_oop over `count` polynomials in groups, so the NTT's second buffer stays bounded (index_build.cu; the caller
+// holds the context lock)
+int ntt_groups(zk_ctx* ctx, int field, const fe* in, size_t in_bs, fe* out, unsigned log_n, size_t count, size_t in_len, int inverse);
+// one commitment of a verifier index: the resident evaluations sub-sampled to d1 (evals[stride i]), plus h on every chunk if masked
+struct IndexCommitment { const fe* evals; uint32_t stride; bool masked; };
+// commit_evaluations_non_hiding of each column over the d1 Lagrange basis (built if the SRS has none), the masked ones + h; out_xy:
+// commitment-major, zk_srs_lagrange_basis_chunks(srs, n) affine points each (index_build.cu; takes the context lock)
+int index_commitments(zk_srs* srs, size_t n, const std::vector<IndexCommitment>& cols, uint64_t* out_xy);
 // zk_msm_partial / zk_msm_finish_gathered without the context lock (the caller holds it)
 int ctx_msm_partial(zk_ctx* ctx, const zk_bases* bases, size_t off, size_t n, const void* scalars, int scalars_are_mont, int window_bits,
                     void* d_out, size_t capacity_points, unsigned* out_c, unsigned* out_groups);

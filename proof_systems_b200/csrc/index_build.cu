@@ -14,7 +14,8 @@
 // zk_index_commitments restates the commitment fields of ProverIndex::verifier_index (kimchi/src/verifier_index.rs:221-300):
 // k_index_gather sub-samples every section to d1 (commit_evaluations_non_hiding, poly-commitment/src/ipa.rs:706-728), the MSMs run
 // as fused batches over the resident Lagrange basis (one per chunk of a chunked basis), and the host adds h to each chunk of the six
-// masked commitments (mask_fixed, verifier_index.rs:179-185).
+// masked commitments (mask_fixed, verifier_index.rs:179-185).  ntt_groups and index_commitments also serve the lookup index
+// (lookup_index.cu).
 #include <algorithm>
 #include <cstring>
 #include <mutex>
@@ -118,7 +119,7 @@ __global__ void __launch_bounds__(256) k_index_gather(const __grid_constant__ In
 }
 
 // the library's NTT over `count` polynomials in groups, so its second buffer stays within NTT_GROUP_BYTES
-static int ntt_groups(zk_ctx* ctx, int field, const fe* in, size_t in_bs, fe* out, unsigned log_n, size_t count, size_t in_len, int inverse) {
+int ntt_groups(zk_ctx* ctx, int field, const fe* in, size_t in_bs, fe* out, unsigned log_n, size_t count, size_t in_len, int inverse) {
     const size_t per = std::max<size_t>(1, NTT_GROUP_BYTES / (sizeof(fe) << log_n));
     for (size_t c0 = 0; c0 < count; c0 += per) {
         const size_t b = std::min(per, count - c0);
@@ -234,11 +235,10 @@ static int index_build_impl(zk_ctx* ctx, const zk_index_header* hdr, const uint8
 }
 
 template <class C>
-static int index_commitments_impl(zk_srs* srs, const zk_index_cache* index, const std::vector<const zk_index_cache::Section*>& secs,
-                                  size_t chunks, uint64_t* out_xy) {
+static int index_commitments_impl(zk_srs* srs, size_t n, const std::vector<IndexCommitment>& cols, size_t chunks, uint64_t* out_xy) {
     using namespace host;
     using HP = typename C::HP;
-    const size_t n = index->hdr.domain_d1_size, k = secs.size();
+    const size_t k = cols.size();
     zk_ctx* ctx = srs->ctx;
     const zk_bases* basis = srs->lagrange.at(n);
     std::vector<uint64_t> jac(12 * k * chunks);
@@ -251,8 +251,8 @@ static int index_commitments_impl(zk_srs* srs, const zk_index_cache* index, cons
             IndexGather g{};
             const unsigned cnt = (unsigned)std::min<size_t>(MAX_GATHER, k - j0);
             for (unsigned j = 0; j < cnt; j++) {
-                g.src[j] = index->payload.at<fe>(secs[j0 + j]->offset - index->lo);
-                g.stride[j] = (uint32_t)(secs[j0 + j]->length / sizeof(fe) / n);
+                g.src[j] = cols[j0 + j].evals;
+                g.stride[j] = cols[j0 + j].stride;
             }
             g.out = d_sc.at<fe>() + j0 * n;
             g.n = n;
@@ -270,17 +270,22 @@ static int index_commitments_impl(zk_srs* srs, const zk_index_cache* index, cons
     haffine h;
     memcpy(&h, srs->h, sizeof(h));
     for (size_t j = 0; j < k; j++) {
-        const bool masked = j >= PERMUTS + COLUMNS && j < PERMUTS + COLUMNS + 6;    // mask_fixed: blinder one, every chunk + h
         for (size_t c = 0; c < chunks; c++) {
             hjac q;
             memcpy(&q, jac.data() + 12 * (j * chunks + c), sizeof(q));
             hxyzz p = from_jacobian<HP>(q);
-            if (masked) p = padd<HP>(p, from_affine<HP>(h));
+            if (cols[j].masked) p = padd<HP>(p, from_affine<HP>(h));     // mask_fixed: blinder one, every chunk + h
             const haffine r = to_affine<HP>(p);
             memcpy(out_xy + 8 * (j * chunks + c), &r, sizeof(r));
         }
     }
     return ZK_OK;
+}
+
+int index_commitments(zk_srs* srs, size_t n, const std::vector<IndexCommitment>& cols, uint64_t* out_xy) {
+    if (int rc = zk_srs_lagrange_basis(srs, n, -1)) return rc;      // get_lagrange_basis (ipa.rs:780-795)
+    const size_t chunks = zk_srs_lagrange_basis_chunks(srs, n);
+    return with_curve(srs->curve, [&](auto c) { return index_commitments_impl<decltype(c)>(srs, n, cols, chunks, out_xy); });
 }
 
 }  // namespace zkb
@@ -341,7 +346,7 @@ int zk_index_commitments(zk_srs* srs, const zk_index_cache* index, uint64_t* out
     for (uint32_t t = 0x20; t <= 0x25; t++) tags.push_back(t);
     for (unsigned b = 0; b < 32; b++)
         if ((index->hdr.optional_selectors_present >> b) & 1) tags.push_back(0x40 + b);
-    std::vector<const zk_index_cache::Section*> secs;
+    std::vector<IndexCommitment> cols;
     for (uint32_t t : tags) {
         const zk_index_cache::Section* s = nullptr;
         for (const auto& o : index->sections)
@@ -349,13 +354,13 @@ int zk_index_commitments(zk_srs* srs, const zk_index_cache* index, uint64_t* out
         if (!s) { zk_set_error("index_commitments: section %#x missing", t); return ZK_ERR_INVALID; }
         const uint64_t len = s->length / sizeof(fe);
         if (len == 0 || len % n || len / n > UINT32_MAX) { zk_set_error("index_commitments: section %#x has %llu elements, not a multiple of %llu", t, (unsigned long long)len, (unsigned long long)n); return ZK_ERR_INVALID; }
-        secs.push_back(s);
+        // the six fixed selectors (generic .. endomul_scalar) are masked
+        cols.push_back({index->payload.at<fe>(s->offset - index->lo), (uint32_t)(len / n), cols.size() >= PERMUTS + COLUMNS && cols.size() < PERMUTS + COLUMNS + 6});
     }
     const size_t chunks = zk_srs_lagrange_basis_chunks(srs, n);
-    *out_points = secs.size() * chunks;
+    *out_points = cols.size() * chunks;
     if (capacity_points < *out_points) { zk_set_error("index_commitments: %zu points do not fit the capacity %zu", *out_points, capacity_points); return ZK_ERR_INVALID; }
-    if (int rc = zk_srs_lagrange_basis(srs, n, -1)) return rc;      // get_lagrange_basis (ipa.rs:780-795)
-    return with_curve(srs->curve, [&](auto c) { return index_commitments_impl<decltype(c)>(srs, index, secs, chunks, out_xy); });
+    return index_commitments(srs, n, cols, out_xy);
 }
 
 }  // extern "C"

@@ -14,7 +14,18 @@ from dataclasses import dataclass
 import numpy as np
 
 from ._lib import (BASE_FIELD, FINAL_CB, FP, FQ, ROUND_CB, SCALAR_FIELD, U_BASE_CB, Context, Handle, IndexHeader, LookupInfo, LookupJoint,
-                   LookupTerm, OpenPoly, OpenTranscript, VerifyProof, ZkError, _fe, _np_u64, _ptr, _u64p, check, jacobian_to_affine, lib)
+                   LookupTable, LookupTerm, OpenPoly, OpenTranscript, RuntimeTableCfg, VerifyProof, ZkError, _fe, _np_u64, _ptr, _u64p, check,
+                   jacobian_to_affine, lib)
+
+
+class LookupIndexError(ZkError):
+    """LookupError of LookupConstraintSystem::create (kimchi/src/circuits/lookup/index.rs:23-36): kind is ID_COLLISION
+    (LookupTableIdCollision), TABLE_ID_ZERO (TableIDZeroMustHaveZeroEntry) or TOO_LONG (LookupTableTooLong); message the reference's"""
+    ID_COLLISION, TABLE_ID_ZERO, TOO_LONG = 1, 2, 3
+
+    def __init__(self, kind: int, message: str):
+        super().__init__(-1, message)
+        self.kind, self.message = kind, message
 
 
 class BlindersDontMatch(ValueError):
@@ -156,6 +167,19 @@ class SRS(Handle):
         return out[: k.value].reshape(-1, chunks, 8)
 
 
+    def lookup_index_commitments(self, index: "IndexCache") -> np.ndarray:
+        """zk_lookup_index_commitments: the commitments of LookupVerifierIndex (kimchi/src/verifier_index.rs:196-215), uint64
+        [count, chunks, 8] affine: lookup_table[0 .. w) and table_ids (masked with blinder one), then the present selectors xor,
+        lookup, range_check, ffmul and runtime_tables_selector."""
+        n = index.header.domain_d1_size
+        chunks = self.lagrange_basis_chunks(n)
+        count = index.section(0x50)[2] + bin(index.header.lookup_selectors_present & 0x3F).count("1")
+        out = np.zeros((count * chunks, 8), dtype=np.uint64)
+        k = ctypes.c_size_t()
+        check(lib().zk_lookup_index_commitments(self._h, index._h, out.ctypes.data_as(_u64p), out.shape[0], ctypes.byref(k)))
+        return out[: k.value].reshape(-1, chunks, 8)
+
+
 class IndexCache(Handle):
     """A cached prover index (kimchi/src/cached_prover_index.rs:26-56, "MINAPK01") resident on the device: zk_index_cache_load parses the
     header and the section table and copies the payload as it lies in the file — raw Montgomery limbs are the device format."""
@@ -169,7 +193,8 @@ class IndexCache(Handle):
         self.ctx, self._h = ctx, ctypes.c_void_p()
         check(_create(ctypes.byref(self._h)))
         self.header = IndexHeader()
-        check(lib().zk_index_cache_header(self._h, ctypes.byref(self.header)))
+        if self._h:                     # IndexCache.build_lookup: no handle when the circuit has no lookup
+            check(lib().zk_index_cache_header(self._h, ctypes.byref(self.header)))
 
     @classmethod
     def build(cls, ctx: Context, fid: int, header, gates: bytes, gate_coeffs: bytes, zero_selectors: bool = False) -> "IndexCache":
@@ -182,6 +207,43 @@ class IndexCache(Handle):
             raise ValueError("gates: a whole number of 60-byte PrunedGate records expected")
         return cls(ctx, _create=lambda out: lib().zk_index_build(ctx._h, fid, ctypes.byref(header), g or None, len(g) // 60, c or None, len(c),
                                                                 int(zero_selectors), out))
+
+    @classmethod
+    def build_lookup(cls, ctx: Context, fid: int, n: int, zk_rows: int, gates: bytes, tables, runtime=None):
+        """zk_lookup_index_build: LookupConstraintSystem::create (kimchi/src/circuits/lookup/index.rs:202-482) on the device.  gates:
+        PrunedGate records as for build; tables: the fixed LookupTables as (id, data), data Montgomery uint64 [width, len, 4] (its
+        columns); runtime: None or the RuntimeTableCfgs as (id, first_column), first_column Montgomery uint64 [len, 4].  Returns
+        (IndexCache, runtime_table_offset or None), or (None, None) when no gate uses a lookup; raises LookupIndexError for the
+        reference's LookupErrors."""
+        g = bytes(gates)
+        if len(g) % 60:
+            raise ValueError("gates: a whole number of 60-byte PrunedGate records expected")
+        keep = []                       # the arrays the structures point into, alive until the call returns
+        fixed = (LookupTable * max(1, len(tables)))()
+        for k, (tid, data) in enumerate(tables):
+            d = np.ascontiguousarray(data, dtype=np.uint64)
+            if d.ndim != 3 or d.shape[2] != 4:
+                raise ValueError("a table's data: uint64 [width, len, 4] expected")
+            keep.append(d)
+            fixed[k] = LookupTable(tid, d.shape[0], d.shape[1], d.ctypes.data if d.size else None)
+        rts = runtime or []
+        rt = (RuntimeTableCfg * max(1, len(rts)))()
+        for k, (tid, col) in enumerate(rts):
+            c = _np_u64(col, (4,)) if len(col) else np.zeros((0, 4), dtype=np.uint64)
+            keep.append(c)
+            rt[k] = RuntimeTableCfg(tid, c.shape[0], c.ctypes.data if c.size else None)
+        err, off = ctypes.c_int(), ctypes.c_uint64()
+
+        def create(out):
+            rc = lib().zk_lookup_index_build(ctx._h, fid, n, zk_rows, g or None, len(g) // 60, fixed, len(tables), rt, len(rts),
+                                             int(runtime is not None), ctypes.byref(err), ctypes.byref(off), out)
+            if rc and err.value:
+                raise LookupIndexError(err.value, lib().zk_last_error().decode(errors="replace"))
+            return rc
+        idx = cls(ctx, _create=create)
+        if not idx._h:
+            return None, None
+        return idx, (off.value if runtime is not None else None)
 
     @classmethod
     def from_file(cls, ctx: Context, path: str, expect_identifier: str | None = None) -> "IndexCache":
