@@ -219,6 +219,10 @@ extern "C" {
                        out_delta_xy: *mut u64, out_z1: *mut u64, out_z2: *mut u64, out_sg_xy: *mut u64) -> c_int;
     pub fn zk_srs_verify(srs: *mut zk_srs, batch: *const zk_verify_proof, n: usize, rng_scalars: *const u64, out_ok: *mut c_int,
                          out_sum_xyz: *mut u64) -> c_int;
+    pub fn zk_srs_accumulator_check(srs: *mut zk_srs, comms_xy: *const u64, n_comms: usize, chals_mont: *const u64, n_chals: usize,
+                                    r_mont: *const u64, out_ok: *mut c_int, out_sum_xyz: *mut u64) -> c_int;
+    pub fn zk_srs_accumulator_generate(srs: *mut zk_srs, num_comms: usize, chals_mont: *const u64, n_chals: usize, out_xy: *mut u64,
+                                       capacity_points: usize, out_points: *mut usize) -> c_int;
 
     pub fn zk_dev_alloc(ctx: *mut zk_ctx, bytes: usize, out: *mut *mut c_void) -> c_int;
     pub fn zk_dev_free(ctx: *mut zk_ctx, d_ptr: *mut c_void) -> c_int;

@@ -19,11 +19,14 @@
 //!   from `cs.gates` and the commitments of its verifier index (kimchi/src/verifier_index.rs:221-300) (`zk_index_build`,
 //!   `zk_index_commitments`); [`index::DeviceLookupIndex`] does the same for the lookup index (kimchi/src/circuits/lookup/index.rs:
 //!   202-482) and the lookup commitments of the verifier index (`zk_lookup_index_build`, `zk_lookup_index_commitments`).
+//! * [`accumulator::batch_dlog_accumulator_check`] and [`accumulator::batch_dlog_accumulator_generate`] are the recursion
+//!   accumulators of poly-commitment/src/utils.rs:204-312 over the resident generators (`zk_srs_accumulator_*`).
 //! * [`lookup::LookupLowering`] builds the lookup argument's joint table, sorted columns and aggregation polynomial
 //!   (kimchi/src/prover.rs:383-673) from the resident witness and the index cache's lookup tables (`zk_lookup_*_dev`).
 //!
 //! Everything called is declared in include/zkb200.h and exported by libzkb200.so; there is no CPU fallback inside the library
 //! (`Ctx::new` fails without a CUDA device) — code that must also run without a GPU keeps using `ipa::SRS`.
+pub mod accumulator;
 pub mod domain;
 pub mod evals;
 pub mod expr;

@@ -323,6 +323,28 @@ typedef struct zk_verify_proof {
 int zk_srs_verify(zk_srs* srs, const zk_verify_proof* batch, size_t n, const uint64_t rng_scalars[8], int* out_ok,
                   uint64_t out_sum_xyz[12]);
 
+/* ------------------------------------------------------------------ recursion accumulators (poly-commitment/src/utils.rs:204-312)
+ * An accumulator is sg = <b_poly_coefficients(chals), g> (commitment.rs:464-476) for one proof's `rounds` challenges.  Challenges
+ * are Montgomery scalars, the accumulators' vectors concatenated in the reference's order; points affine Montgomery (identity =
+ * zeros), not checked to lie on the curve (the reference relies on deserialisation).  With k accumulators (n_comms / num_comms),
+ * rounds = n_chals / k as in the reference, and the calls fail where it panics: ZK_ERR_INVALID for k = 0 with challenges, for
+ * n_chals < k (rounds = 0) and for n_chals not a multiple of rounds.  Zero challenges are allowed.  Both calls hold the context
+ * lock and run on the context's stream; the challenge polynomials are expanded on the device (csrc/bpoly.cuh).
+ *
+ * zk_srs_accumulator_check     batch_dlog_accumulator_check (utils.rs:212-273, kimchi-stubs/src/urs_utils.rs:10-69):
+ *     *out_ok = 1 iff  <g, -sum_i r^i s_i> + sum_i r^i comms_i  is the identity, s_i the coefficients of chunk i of the challenges
+ *     (only the first k chunks enter, as the reference's zip does).  r_mont: the scalar the reference draws from OsRng (r = 0
+ *     checks the first accumulator alone).  ZK_ERR_LENGTH when 2^rounds != |g| (assert_eq!(terms.len(), n)).  k = 0 without
+ *     challenges: *out_ok = 1.  out_sum_xyz (optional): the sum, Jacobian.
+ * zk_srs_accumulator_generate  batch_dlog_accumulator_generate (utils.rs:275-312, urs_utils.rs:71-101): one accumulator per chunk
+ *     of `rounds` challenges — n_chals / rounds of them, which exceeds num_comms when n_chals / num_comms does not divide evenly
+ *     (num_comms = 3 with 8 challenges: rounds 2, 4 points) — each MSM over min(2^rounds, |g|) generators as msm_bigint truncates.
+ *     *out_points receives the count first; more than capacity_points: ZK_ERR_INVALID.  out_xy: the points, affine. */
+int zk_srs_accumulator_check(zk_srs* srs, const uint64_t* comms_xy, size_t n_comms, const uint64_t* chals_mont, size_t n_chals,
+                             const uint64_t r_mont[4], int* out_ok, uint64_t out_sum_xyz[12]);
+int zk_srs_accumulator_generate(zk_srs* srs, size_t num_comms, const uint64_t* chals_mont, size_t n_chals, uint64_t* out_xy,
+                                size_t capacity_points, size_t* out_points);
+
 /* ------------------------------------------------------------------ d8 pipeline, first pointwise evaluator (SURVEY.md §8f row 3)
  * The permutation part of the quotient polynomial in evaluation form over d8 (m = 2^log_m points), all operands resident on the
  * device — kimchi/src/circuits/polynomials/permutation.rs:223-357, `perm`:

@@ -11,6 +11,7 @@ reference's interfaces on this path, with the reference's names:
     LagrangeBasisEvaluations.new / evaluate / evaluate_boolean             kimchi/src/lagrange_basis_evaluations.rs:72-258
     IndexCache.build / SRS.index_commitments                               kimchi/src/circuits/constraints.rs:510-760, verifier_index.rs:221-300
     IndexCache.build_lookup / SRS.lookup_index_commitments                 kimchi/src/circuits/lookup/index.rs:202-482, verifier_index.rs:196-215
+    batch_dlog_accumulator_check / batch_dlog_accumulator_generate         poly-commitment/src/utils.rs:204-312
 
 There is no CPU fallback anywhere in this package: importing it without the built library, or creating a Context
 without a CUDA device, raises.
@@ -21,4 +22,5 @@ from ._lib import (  # noqa: F401
 )
 from .host import (  # noqa: F401
     SRS, BatchEvaluationProof, ExprProgram, IndexCache, IpaRounds, LookupIndexError, LagrangeBasisEvaluations, LookupSpec, OpeningProof, PolyComm, Radix2EvaluationDomain, srs_open, srs_verify,
+    batch_dlog_accumulator_check, batch_dlog_accumulator_generate,
 )

@@ -144,6 +144,8 @@ def lib() -> ctypes.CDLL:
     L.zk_lookup_index_build.argtypes = [vp, i, ctypes.c_uint64, ctypes.c_uint64, vp, sz, ctypes.POINTER(LookupTable), sz,
                                         ctypes.POINTER(RuntimeTableCfg), sz, i, ctypes.POINTER(i), ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(vp)]
     L.zk_lookup_index_commitments.argtypes = [vp, vp, _u64p, sz, ctypes.POINTER(sz)]
+    L.zk_srs_accumulator_check.argtypes = [vp, vp, sz, vp, sz, vp, ctypes.POINTER(i), vp]
+    L.zk_srs_accumulator_generate.argtypes = [vp, sz, vp, sz, vp, sz, ctypes.POINTER(sz)]
     return L
 
 

@@ -115,7 +115,9 @@ struct zk_ctx {
     zkb::DevScratch d_flag;              // zk_poly_divide_by_vanishing_dev: remainder flag
     zkb::DevScratch d_expr;              // zk_expr_eval_dev: program | constants | column table
     zkb::DevScratch d_ipa;               // zk_srs_open: the rounds' state (a, b, challenge products, expanded scalars), kept between calls
-    zkb::DevScratch d_verify;            // zk_srs_verify: s vector | challenge tables | proof points and their scalars
+    zkb::DevScratch d_verify;            // zk_srs_verify: s vector | challenge tables | proof points and their scalars;
+                                         // zk_srs_accumulator_check / _generate (never at once: both hold `mu`): the s vector or
+                                         // one group's expanded vectors | challenge tables | weights | commitments and their scalars
     zkb::DevScratch d_evals;             // zk_lagrange_evaluate_dev / zk_poly_evaluate_chunks_dev: descriptors | partial sums | results
     zkb::DevScratch d_ft;                // zk_prover_ft_dev: f over d1 | term descriptors | length counter
     zkb::DevScratch d_perm;              // zk_perm_aggreg_dev: den, then num / den over d1 | block products | final-value flag

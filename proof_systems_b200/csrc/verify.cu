@@ -4,7 +4,7 @@
 // it with zero.  Here it is split in two:
 //   * the g part: S[j] = sum_i sg_rand_base^i s_i[j], s_i = b_poly_coefficients(chal_i) (commitment.rs:464-476: bit t of j selects
 //     chal_i[k_i - 1 - t]).  Per proof, a table of the products over the low L bits of j and one over the high K - L bits (the
-//     weight folded into the high table) are built by k_verify_tables; k_verify_s then costs one product and one addition per
+//     weight folded into the high table) are built by k_bpoly_tables; k_bpoly_sum then costs one product and one addition per
 //     (proof, j).  Two launches for the whole batch, whatever its size.  S runs through the fused MSM pipeline over the resident
 //     generator table (ctx_msm_many, Montgomery scalars).
 //   * the proof points: h, then per proof sg, U (its two scalars merged), L_j, R_j, the commitment chunks, delta — about
@@ -20,49 +20,12 @@
 
 #include "../../include/zkb200.h"
 #include "ctx.hpp"
+#include "bpoly.cuh"
 #include "msm.cuh"
 
 using namespace zkb;
 
 namespace zkb {
-
-// Per proof i (blockIdx-linear index over B x (2^L + 2^H) entries):
-//   lo[i][e] = prod_{t < L, bit t of e} rev[i][t]           hi[i][e] = w[i] * prod_{t < H, bit t of e} rev[i][L + t]
-// rev[i][t] = chal_i[k_i - 1 - t] for t < k_i and 0 above, so the entries of j >= 2^k_i vanish (the proof's s covers 2^k_i entries)
-template <class FS>
-__global__ void k_verify_tables(const fe* __restrict__ rev, const fe* __restrict__ w, unsigned B, unsigned K, unsigned L, fe* lo, fe* hi) {
-    const unsigned H = K - L;
-    const size_t per = ((size_t)1 << L) + ((size_t)1 << H);
-    const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= per * B) return;
-    const unsigned i = (unsigned)(idx / per);
-    size_t e = idx % per;
-    const fe* r = rev + (size_t)i * K;
-    if (e < ((size_t)1 << L)) {
-        fe v = fe_one<FS>();
-        for (unsigned t = 0; t < L; t++)
-            if ((e >> t) & 1) v = fe_mul<FS>(v, load_fe_nc(r + t));
-        store_fe(lo + ((size_t)i << L) + e, v);
-    } else {
-        e -= (size_t)1 << L;
-        fe v = load_fe_nc(w + i);
-        for (unsigned t = 0; t < H; t++)
-            if ((e >> t) & 1) v = fe_mul<FS>(v, load_fe_nc(r + L + t));
-        store_fe(hi + ((size_t)i << H) + e, v);
-    }
-}
-
-// S[j] = sum_i lo[i][j mod 2^L] * hi[i][j >> L],  j < len
-template <class FS>
-__global__ void k_verify_s(const fe* __restrict__ lo, const fe* __restrict__ hi, unsigned B, unsigned L, unsigned H, fe* S, size_t len) {
-    const size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= len) return;
-    const size_t jl = j & (((size_t)1 << L) - 1), jh = j >> L;
-    fe acc = fe_zero();
-    for (unsigned i = 0; i < B; i++)
-        acc = fe_add<FS>(acc, fe_mul<FS>(load_fe_nc(lo + ((size_t)i << L) + jl), load_fe_nc(hi + ((size_t)i << H) + jh)));
-    store_fe(S + j, acc);
-}
 
 template <class C>
 static int verify_impl(zk_srs* srs, const zk_verify_proof* batch, size_t B, const uint64_t* rng, int* out_ok, uint64_t* out_sum_xyz) {
@@ -194,9 +157,9 @@ static int verify_impl(zk_srs* srs, const zk_verify_proof* batch, size_t B, cons
     ZK_CUDA(cudaMemcpyAsync(d_sc, sc.data(), n_pts * sizeof(fe), cudaMemcpyHostToDevice, st));
     ZK_CUDA(cudaMemcpyAsync(d_pts, pts.data(), n_pts * sizeof(affine_t), cudaMemcpyHostToDevice, st));
     const size_t n_tab = n_lo + n_hi;
-    k_verify_tables<FS><<<(unsigned)((n_tab + 127) / 128), 128, 0, st>>>(d_rev, d_w, (unsigned)B, K, L, d_lo, d_hi);
+    k_bpoly_tables<FS><<<(unsigned)((n_tab + 127) / 128), 128, 0, st>>>(d_rev, d_w, (unsigned)B, K, L, d_lo, d_hi);
     ZK_CUDA(cudaGetLastError());
-    k_verify_s<FS><<<(unsigned)((len + 127) / 128), 128, 0, st>>>(d_lo, d_hi, (unsigned)B, L, H, d_S, len);
+    k_bpoly_sum<FS><<<(unsigned)((len + 127) / 128), 128, 0, st>>>(d_lo, d_hi, (unsigned)B, L, H, d_S, len);
     ZK_CUDA(cudaGetLastError());
     ctx->launches += 2;
     if (trace) ZK_CUDA(cudaStreamSynchronize(st));

@@ -9,6 +9,7 @@ Names, argument meaning and error behaviour follow the reference so that the par
 from __future__ import annotations
 
 import ctypes
+import os
 from dataclasses import dataclass
 
 import numpy as np
@@ -391,6 +392,56 @@ def srs_verify(srs, batch, rand_base, sg_rand_base, return_sum: bool = False):
     if not return_sum:
         return bool(ok.value)
     return bool(ok.value), jacobian_to_affine(srs.curve, out)
+
+
+# the scalar fields' moduli (curves/src/pasta/fields/fp.rs, fq.rs)
+_MODULUS = {FP: 0x40000000000000000000000000000000224698fc094cf91b992d30ed00000001,
+            FQ: 0x40000000000000000000000000000000224698fc0994a8dd8c46eb2100000001}
+
+
+def _os_scalar(field: int) -> np.ndarray:
+    """F::rand(&mut OsRng): uniform below the modulus by rejection, from the OS's randomness.  Montgomery limbs [4]: the Montgomery
+    form of a uniform element is itself uniform below the modulus."""
+    m = _MODULUS[field]
+    while True:
+        x = int.from_bytes(os.urandom(32), "little") >> 1
+        if x < m:
+            return np.array([(x >> (64 * i)) & 0xFFFFFFFFFFFFFFFF for i in range(4)], dtype=np.uint64)
+
+
+def _rows(a, tail):
+    """a as contiguous uint64 [-1, *tail], also when empty"""
+    return _np_u64(a, tail) if np.size(a) else np.zeros((0,) + tail, dtype=np.uint64)
+
+
+def batch_dlog_accumulator_check(srs, comms, chals, r=None, return_sum: bool = False):
+    """batch_dlog_accumulator_check (poly-commitment/src/utils.rs:212-273) through zk_srs_accumulator_check: True iff the k
+    accumulators comms [k, 8] equal <b_poly_coefficients(chals_i), g> for the first k chunks of `rounds = len(chals) / k`
+    challenges (chals [n, 4], Montgomery).  r: the scalar the reference draws from OsRng (Montgomery [4]); None draws one from the
+    OS's randomness.  With return_sum, also the affine point [8] the check compares with zero.  Where the reference panics the
+    library refuses, raised as ZkError."""
+    c, ch = _rows(comms, (8,)), _rows(chals, (4,))
+    rr = _os_scalar(SCALAR_FIELD[srs.curve]) if r is None else _fe(r)
+    ok = ctypes.c_int(0)
+    out = np.zeros(12, dtype=np.uint64)
+    check(lib().zk_srs_accumulator_check(srs._h, _ptr(c) if c.size else None, c.shape[0], _ptr(ch) if ch.size else None, ch.shape[0],
+                                         _ptr(rr), ctypes.byref(ok), _ptr(out)))
+    if not return_sum:
+        return bool(ok.value)
+    return bool(ok.value), jacobian_to_affine(srs.curve, out)
+
+
+def batch_dlog_accumulator_generate(srs, num_comms: int, chals) -> np.ndarray:
+    """batch_dlog_accumulator_generate (poly-commitment/src/utils.rs:275-312) through zk_srs_accumulator_generate: one accumulator
+    <b_poly_coefficients(chunk), g> per chunk of `rounds = len(chals) / num_comms` challenges (chals [n, 4], Montgomery), as uint64
+    [n / rounds, 8] affine.  Where the reference panics the library refuses, raised as ZkError."""
+    ch = _rows(chals, (4,))
+    n = ch.shape[0]
+    cap = n // (n // num_comms) if num_comms and n >= num_comms else 0
+    out = np.zeros((max(cap, 1), 8), dtype=np.uint64)
+    got = ctypes.c_size_t(0)
+    check(lib().zk_srs_accumulator_generate(srs._h, num_comms, _ptr(ch) if ch.size else None, n, _ptr(out), cap, ctypes.byref(got)))
+    return out[: got.value]
 
 
 class IpaRounds(Handle):
